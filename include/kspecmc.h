@@ -112,14 +112,11 @@ typedef struct {
  * "gpus":N (N > 1: this ONE context drives N GPUs of the process -- fingerprint-sharded, one host thread per GPU
  *   inside kmc_run, peers mapped with cudaDeviceEnablePeerAccess; kmc_stats / kmc_violation / kmc_trace_* then
  *   report the whole job),
- * "overlap":false (single GPU: the hash-probe kernel of chunk i runs on a second stream under the expand kernel of
- *   chunk i+1), "chunk_states":N (frontier states per expand/insert launch pair), "prefetch":false (experiment),
  * "spill":false (the state store is a ring over the live BFS window, max_states slots rounded down to a power of
  *   two; older levels move to host memory -- TLC's DiskStateQueue),
  * "checkpoint_dir":"d", "checkpoint_minutes":M (TLC -checkpoint: states + parent links + counters written at a level
  *   boundary at most every M minutes, 0 = every level), "recover":"d" (TLC -recover: continue from that checkpoint;
- *   the set is rebuilt from the stored states),
- * "one_phase":false (comparison only: the round-1 one-phase expand kernel; needs a -DKMC_ONE_PHASE library).  */
+ *   the set is rebuilt from the stored states).  */
 int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out);
 void kmc_destroy(kmc_ctx* ctx);
 int kmc_model_info(const kmc_ctx* ctx, kmc_model_info_t* out);

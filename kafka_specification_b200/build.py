@@ -75,21 +75,8 @@ def model_dir(name: str) -> str:
     return os.path.join(BUILD, "models", name)
 
 
-# build variants: extra nvcc flags and a library-name suffix.  The default build carries the two-phase expand
-# kernel only (-DKMC_NO_ONE_PHASE drops the one-phase form of the lowered Next from the translation unit);
-# "1p" adds the round-1 one-phase kernel for A/B measurements (option "one_phase": true).
-VARIANTS = {
-    "": ["-DKMC_NO_ONE_PHASE"],
-    "1p": ["-DKMC_ONE_PHASE"],
-    "b512": ["-DKMC_NO_ONE_PHASE", "-DEXPAND_BLOCK_THREADS=512", "-DEXPAND_CTAS_PER_SM=2"],    # two 512-thread CTAs per SM
-    "bs4": ["-DKMC_NO_ONE_PHASE", "-DKMC_BUCKET_SLOTS=4"],
-    "b768": ["-DKMC_NO_ONE_PHASE", "-DEXPAND_BLOCK_THREADS=768"],      # 24 warps: leaves registers for K2 blocks (overlap)
-    "b512x1": ["-DKMC_NO_ONE_PHASE", "-DEXPAND_BLOCK_THREADS=512"],                                   # 64-byte buckets of 16-byte keys
-}
-
-
-def model_lib_path(name: str, variant: str = "") -> str:
-    return os.path.join(model_dir(name), f"libkmc_{name}{'.' + variant if variant else ''}.so")
+def model_lib_path(name: str) -> str:
+    return os.path.join(model_dir(name), f"libkmc_{name}.so")
 
 
 def _engine_stamp() -> str:
@@ -100,14 +87,14 @@ def _engine_stamp() -> str:
     return h.hexdigest()[:16]
 
 
-def lower_to_dir(module: str, cfg_path: str, name: str, **lower_kw):
+def lower_to_dir(module: str, cfg_path: str, name: str):
     """Lower and write model.h / model.json; returns the LoweredModel."""
     import time
     from .lower.model import lower_model
     with open(cfg_path) as f:
         cfg_text = f.read()
     t0 = time.time()
-    m = lower_model(module, tla_search_dirs(), cfg_text, name=name, **lower_kw)
+    m = lower_model(module, tla_search_dirs(), cfg_text, name=name)
     lower_seconds = time.time() - t0
     d = model_dir(name)
     os.makedirs(d, exist_ok=True)
@@ -124,25 +111,31 @@ def lower_to_dir(module: str, cfg_path: str, name: str, **lower_kw):
     return m
 
 
-def compile_model(name: str, force: bool = False, verbose_ptxas: bool = True, variant: str = "",
-                  extra_flags: list[str] | None = None) -> str:
+def _nvcc_cmd(hdr: str, out_so: str) -> list[str]:
+    """nvcc of the engine with a lowered header.  The engine runs the two-phase form of the lowered Next only, so
+    -DKMC_NO_ONE_PHASE drops the one-phase form from the translation unit (it would only add nvcc time)."""
+    return [nvcc_path(), *NVCC_ARCH, "-lineinfo", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
+            "-diag-suppress", "177", "-DKMC_NO_ONE_PHASE",
+            f"-I{INCLUDE}", "-include", hdr, os.path.join(CSRC, "kmc_engine.cu"), "-o", out_so]
+
+
+def compile_model(name: str, force: bool = False, verbose_ptxas: bool = True) -> str:
     d = model_dir(name)
     hdr = os.path.join(d, "model.h")
-    so = model_lib_path(name, variant)
-    stamp_file = os.path.join(d, f"build{'.' + variant if variant else ''}.stamp")
+    so = model_lib_path(name)
+    stamp_file = os.path.join(d, "build.stamp")
     with open(hdr, "rb") as f:
         stamp = hashlib.sha256(f.read()).hexdigest()[:16] + ":" + _engine_stamp()
     if not force and os.path.exists(so) and os.path.exists(stamp_file) and open(stamp_file).read() == stamp:
         return so
-    cmd = [nvcc_path(), *NVCC_ARCH, "-lineinfo", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
-           "-diag-suppress", "177", *VARIANTS[variant], *(extra_flags or []),
-           f"-I{INCLUDE}", "-include", hdr, os.path.join(CSRC, "kmc_engine.cu"), "-o", so]
+    cmd = _nvcc_cmd(hdr, so)
     if verbose_ptxas:
         cmd[1:1] = ["-Xptxas", "-v"]
     import time
     t0 = time.time()
-    _run(cmd, log=os.path.join(d, f"nvcc{'.' + variant if variant else ''}.log"))
-    with open(os.path.join(d, f"nvcc{'.' + variant if variant else ''}.log"), "a") as f:
+    log = os.path.join(d, "nvcc.log")
+    _run(cmd, log=log)
+    with open(log, "a") as f:
         f.write(f"nvcc wall time: {time.time() - t0:.1f} s\n")
     with open(stamp_file, "w") as f:
         f.write(stamp)
@@ -151,9 +144,7 @@ def compile_model(name: str, force: bool = False, verbose_ptxas: bool = True, va
 
 def compile_model_to(name: str, out_so: str) -> str:
     """Plain nvcc of the prebuilt lowered header into `out_so` (no stamp, no log): the cold-start timing of bench.py."""
-    hdr = os.path.join(model_dir(name), "model.h")
-    _run([nvcc_path(), *NVCC_ARCH, "-lineinfo", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC", "-diag-suppress", "177",
-          *VARIANTS[""], f"-I{INCLUDE}", "-include", hdr, os.path.join(CSRC, "kmc_engine.cu"), "-o", out_so])
+    _run(_nvcc_cmd(os.path.join(model_dir(name), "model.h"), out_so))
     return out_so
 
 

@@ -1,29 +1,28 @@
 // kmc_engine.cu -- the BFS frontier-expansion engine, compiled once per lowered model:
 //
-//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -shared \
-//        -Xcompiler -fPIC -include <model>.h kmc_engine.cu -o libkmc_<model>.so
+//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -shared -Xcompiler -fPIC \
+//        -DKMC_NO_ONE_PHASE -include <model>.h kmc_engine.cu -o libkmc_<model>.so
 //
 // It replaces TLC's Worker next-state loop, FPSet and StateQueue (SURVEY.md section 8):
 //
-//   k_expand  (K1)  lowered Next over the frontier.  The unrolled Next is hundreds of KB of SASS, so it
-//                   is cut into NUM_GROUPS groups; one 1024-thread CTA per SM sweeps one group at a
-//                   time over a tile of states (all warps in the same group => the group's code stays in
-//                   the instruction cache).  Successor rows (state words + parent/action word) are
-//                   staged per warp in shared memory and flushed in bulk: into the local candidate
-//                   buffer (one rank), into per-owner regions (NCCL exchange), or -- fused exchange --
-//                   straight into the owner rank's inbox through a CUDA-IPC peer mapping (NVLink stores).
-//   k_insert  (K2)  one thread per candidate: 64-bit fingerprint (of the orbit representative under
-//                   SYMMETRY), open-addressing hash set in HBM with 32-byte buckets (4 fingerprints =
-//                   one DRAM sector, two 128-bit loads), CAS insertion, warp ballot/popc compaction of
+//   k_expand  (K1)  lowered Next over the frontier, in two phases per site group: every lane evaluates the
+//                   complete path conditions of its states (site_mask), then warps run the straight-line
+//                   bodies of the enabled (state, site) pairs one site at a time (site_body).  Successor
+//                   rows (state words + parent/action word) are staged per warp in shared memory and
+//                   flushed in bulk: into the local candidate buffer (one rank), into per-owner regions
+//                   (NCCL exchange), or -- fused exchange -- straight into the owner rank's inbox through
+//                   a peer mapping (NVLink stores).
+//   k_insert  (K2)  one thread per candidate: identity (see state_ident), open-addressing hash set in HBM
+//                   with 32-byte buckets (one DRAM sector), CAS insertion, warp ballot/popc compaction of
 //                   the winners into the state store (= next frontier), parent link.  k_insert_inbox is
 //                   the same over the regions the peers filled.
 //   k_invariants (K3) the cfg's INVARIANTs on the new states of a level (compacted => every lane busy).
 //                   Violating states (rare, terminal) go to a small ring; the host reports the one with
 //                   the smallest fingerprint, so the counterexample is deterministic.
-//   k_expand2       opt-in two-phase form of K1 (guard masks, CTA-wide compaction, bodies); measured
-//                   slower, see DESIGN.md section 4.
 //
-// HBM layout (per rank):   table  u64[2^table_log2]            fingerprints, 0 = empty
+// DESIGN.md sections 3-4 give the layout, the kernels and their measurements.
+//
+// HBM layout (per rank):   table  2^table_log2 slots           8-byte fingerprints or 16-byte keys (see KEY128)
 //                          store  u64[max_states][W]           all distinct states, BFS order;
 //                                                              level k is a contiguous range
 //                          parent u64[max_states]              parent ref | action << 56
@@ -83,10 +82,7 @@ __host__ __device__ __forceinline__ uint64_t fmix64(uint64_t x) {
 // The 64-bit fingerprint also picks the bucket and the owner rank and orders counterexamples.
 static constexpr bool KEY128 = (W >= 2);
 static constexpr bool EXACT_SET = EXACT64 || (W == 2 && !M::ALL_ONES_POSSIBLE);
-#ifndef KMC_BUCKET_SLOTS
-#define KMC_BUCKET_SLOTS 2            // 16-byte slots per bucket: 2 = one 32 B sector, 4 = one 64 B DRAM burst
-#endif
-static constexpr int BUCKET_SLOTS = KEY128 ? KMC_BUCKET_SLOTS : 4;
+static constexpr int BUCKET_SLOTS = KEY128 ? 2 : 4;      // one 32 B sector per bucket
 static constexpr int SLOT_BYTES = KEY128 ? 16 : 8;
 
 struct alignas(16) Key128 {
@@ -194,8 +190,6 @@ struct Params {
   uint32_t rank, world;
   uint32_t check_deadlock;
   uint32_t count_actions;
-  uint32_t prefetch;        // K1 issues an L2 prefetch of every candidate's first bucket (see flush_stage)
-  uint32_t cand_slot;       // single rank: which half of the candidate buffer (and which counter) this launch uses
   // fused exchange (world > 1, after kmc_shard_open_peers): every rank's inbox, mapped into this
   // process through CUDA IPC.  An inbox is two buffers (double buffering); a buffer is an 8-word
   // header (rows sent by each source rank) followed by world regions of region_rows rows.
@@ -232,9 +226,6 @@ __device__ __noinline__ void record_violation(const Params& p, const State& s, u
   row[W + 2] = inv;
 }
 
-// ----------------------------------------------------------------------------------------
-// K1: expand
-// ----------------------------------------------------------------------------------------
 // ----------------------------------------------------------------------------------------
 // K2 primitives: the fingerprint set
 // ----------------------------------------------------------------------------------------
@@ -405,13 +396,7 @@ __device__ __forceinline__ void insert_row(const Params& p, const State& s, uint
 // and -- multi-rank -- the owner computation (a fingerprint) done with all 32 lanes busy instead
 // of inside the emit site.  The stage is addressed through 32-bit shared-window addresses and
 // st.shared / atom.shared so that no generic-address store (ST + QSPC) is ever generated.
-#ifndef EXPAND_BLOCK_THREADS
-#define EXPAND_BLOCK_THREADS 1024
-#endif
-#ifndef EXPAND_CTAS_PER_SM
-#define EXPAND_CTAS_PER_SM 1          // 2 (with 512 threads): one CTA's barrier waits are covered by the other CTA
-#endif
-static constexpr int EXPAND_BLOCK = EXPAND_BLOCK_THREADS;
+static constexpr int EXPAND_BLOCK = 1024;        // one CTA per SM
 static constexpr int NWARPS = EXPAND_BLOCK / 32;
 static constexpr int STAGE_ROWS = 64;            // rows per warp; a body pass adds <= 32, a flush empties it
 static constexpr int STAGE_FLUSH = 32;           // flush once at least this many rows are staged
@@ -467,25 +452,13 @@ __device__ __forceinline__ void flush_stage(const Params& p, uint32_t wbuf, uint
   unsigned lane = lane_id();
   if (p.world == 1) {
     unsigned long long base = 0;
-    if (lane == 0) base = atomicAdd(&p.ctr->cand_count[p.cand_slot], (unsigned long long)n);
+    if (lane == 0) base = atomicAdd(&p.ctr->cand_count[0], (unsigned long long)n);
     base = __shfl_sync(0xffffffffu, base, 0);
     if (base + n > p.region_rows) {
       failed = KMC_FAIL_CAND_FULL;
     } else {
       uint64_t* dst = p.cand + base * ROW;
       for (unsigned k = lane; k < n * ROW; k += 32) dst[k] = lds64(wbuf + k * 8);      // coalesced
-      if (p.prefetch && !M::HAS_SYMMETRY) {
-        // Software pipelining across kernels through the L2: the bucket this candidate will probe in K2 is
-        // requested now, while K1 still has integer work to hide the DRAM latency behind.  With frontier chunks
-        // sized so that a chunk's buckets fit the 50 MB L2, K2 then probes L2-resident sectors.
-        for (unsigned r = lane; r < n; r += 32) {
-          State t;
-#pragma unroll
-          for (int q = 0; q < W; ++q) t.w[q] = lds64(wbuf + (r * ROW + q) * 8);
-          const char* a = bucket_addr(p.table, bucket_of(fingerprint(t), p.bucket_mask));
-          asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(a));
-        }
-      }
     }
   } else {
     for (unsigned r0 = 0; r0 < n; r0 += 32) {
@@ -513,11 +486,6 @@ struct CandSink {
   unsigned long long* action_counts;   // per-action counters (global memory), or nullptr
   int n;
   int failed;
-#ifdef KMC_ONE_PHASE
-  uint64_t* cand;                      // one-phase comparison kernel only (single rank): overflow rows go straight
-  unsigned long long* cand_count;      // to the candidate buffer
-  uint64_t region_rows;
-#endif
 
   __device__ __forceinline__ void emit(const State& s, int action) {
     ++n;
@@ -535,20 +503,7 @@ struct CandSink {
       for (int i = 0; i < W; ++i) sts64(row + i * 8, s.w[i]);
       sts64(row + W * 8, meta);
     } else {
-#ifdef KMC_ONE_PHASE
-      if (cand != nullptr) {           // one-phase kernel: a burst of emits between two flushes
-        unsigned long long gpos = atomicAdd(cand_count, 1ull);
-        if (gpos >= region_rows) {
-          failed = KMC_FAIL_CAND_FULL;
-        } else {
-          uint64_t* grow = cand + gpos * ROW;
-#pragma unroll
-          for (int i = 0; i < W; ++i) grow[i] = s.w[i];
-          grow[W] = meta;
-        }
-      } else
-#endif
-      // two-phase kernel: cannot happen (a body pass adds <= 32 rows to a stage that is flushed at >= STAGE_FLUSH)
+      // cannot happen (a body pass adds <= 32 rows to a stage that is flushed at >= STAGE_FLUSH)
       failed = KMC_FAIL_CAND_FULL;
     }
     if (action_counts != nullptr && action < 64) atomicAdd(action_counts + action, 1ull);
@@ -579,7 +534,7 @@ __device__ __forceinline__ void load_state(State& s, const uint64_t* src) {
 // ----------------------------------------------------------------------------------------
 static constexpr int STAGE_BYTES = NWARPS * STAGE_ROWS * ROW * 8;
 static constexpr int FIXED_SMEM_BYTES = STAGE_BYTES + LIST_CAP * 2 + (4 * MAX_GROUP_SITES + NWARPS + 8) * 4;
-static constexpr int SPT_FIT = (227 * 1024 / EXPAND_CTAS_PER_SM - 1024 - FIXED_SMEM_BYTES) / (EXPAND_BLOCK * W * 8);
+static constexpr int SPT_FIT = (227 * 1024 - 1024 - FIXED_SMEM_BYTES) / (EXPAND_BLOCK * W * 8);
 static constexpr int SPT = SPT_FIT > 4 ? 4 : SPT_FIT;
 static_assert(SPT >= 1, "state too wide for the expand kernel's shared-memory tile");
 static constexpr int TILE = EXPAND_BLOCK * SPT;
@@ -745,11 +700,7 @@ struct SiteGroupRunner {
 #pragma unroll
           for (int q = 0; q < W; ++q) s.w[q] = lds64(c.tile + (slot * W + q) * 8);
           CandSink sink{(c.first + c.tile_base + slot) | ((uint64_t)p.rank << 40), c.wbuf, c.wcnt,
-                        p.count_actions ? p.ctr->action_counts : nullptr, 0, 0
-#ifdef KMC_ONE_PHASE
-                        , nullptr, nullptr, 0
-#endif
-          };
+                        p.count_actions ? p.ctr->action_counts : nullptr, 0, 0};
           SiteDispatch<BEGIN, END>::run(k + BEGIN, s, sink);
           failed |= sink.failed;
         }
@@ -765,7 +716,7 @@ struct SiteGroupRunner<M::NUM_SITE_GROUPS> {
   static __device__ __forceinline__ void run(const Params&, const TileCtx&, unsigned (&)[SPT], int&) {}
 };
 
-__global__ void __launch_bounds__(EXPAND_BLOCK, EXPAND_CTAS_PER_SM) k_expand(Params p, uint64_t first, uint64_t count, unsigned tile_states) {
+__global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t first, uint64_t count, unsigned tile_states) {
   extern __shared__ __align__(16) uint64_t smem[];   // tile | stage | list | cnt[2][64] | cur[64] | seg[64] | wcnt[NWARPS]
   const int warp = threadIdx.x >> 5;
   TileCtx c;
@@ -840,92 +791,6 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, EXPAND_CTAS_PER_SM) k_expand(Par
     if (failed) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)failed);
   }
 }
-
-#ifdef KMC_ONE_PHASE
-// ----------------------------------------------------------------------------------------
-// K1, one-phase (round 1): comparison build only (-DKMC_ONE_PHASE, option "one_phase").  The
-// lowered Next is cut into NUM_GROUPS groups of ~1k instructions and the CTA sweeps ONE group at
-// a time over a tile of EXPAND_BLOCK x spt states (__syncthreads between groups keeps all warps
-// of the SM in the same group, so a fetched instruction line serves every warp).
-// ----------------------------------------------------------------------------------------
-static constexpr int EXPAND_SPT1 = 4;
-template <int G>
-struct GroupRunner {
-  static __device__ __forceinline__ void run(const Params& p, uint64_t first, uint64_t tile_base, uint64_t count,
-                                              int spt, unsigned (&nsucc)[EXPAND_SPT1], int& failed, uint32_t wbuf, uint32_t wcnt) {
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < EXPAND_SPT1; ++j) {
-      if (j < spt) {
-        uint64_t i = tile_base + (uint64_t)j * EXPAND_BLOCK + threadIdx.x;
-        if (i < count) {
-          State s;
-          load_state(s, p.store + ((first + i) & p.store_mask) * W);
-          CandSink sink{(first + i) | ((uint64_t)p.rank << 40), wbuf, wcnt, p.count_actions ? p.ctr->action_counts : nullptr, 0, 0,
-                        p.world == 1 ? p.cand : nullptr, &p.ctr->cand_count[p.cand_slot], p.region_rows};
-          M::expand_group(M::GroupTag<G>{}, s, sink);
-          nsucc[j] += (unsigned)sink.n;
-          failed |= sink.failed;
-        }
-        flush_stage(p, wbuf, wcnt, false, failed);
-      }
-    }
-    GroupRunner<G + 1>::run(p, first, tile_base, count, spt, nsucc, failed, wbuf, wcnt);
-  }
-};
-template <>
-struct GroupRunner<M::NUM_GROUPS> {
-  static __device__ __forceinline__ void run(const Params&, uint64_t, uint64_t, uint64_t, int, unsigned (&)[EXPAND_SPT1], int&,
-                                              uint32_t, uint32_t) {}
-};
-
-__global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand1(Params p, uint64_t first, uint64_t count, int spt) {
-  extern __shared__ __align__(16) uint64_t smem[];          // [warps][STAGE_ROWS][ROW] then [warps] counters
-  const int warp = threadIdx.x >> 5;
-  const uint32_t wbuf = smem_addr(smem) + warp * (STAGE_ROWS * ROW * 8);
-  const uint32_t wcnt = smem_addr(smem) + STAGE_BYTES + warp * 4;
-  if (lane_id() == 0) sts32(wcnt, 0u);
-  __syncwarp();
-  unsigned long long gen = 0, dead = 0;
-  unsigned maxfan = 0;
-  int failed = 0;
-  const uint64_t tile = (uint64_t)EXPAND_BLOCK * spt;
-  for (uint64_t tile_base = (uint64_t)blockIdx.x * tile; tile_base < count; tile_base += (uint64_t)gridDim.x * tile) {
-    unsigned nsucc[EXPAND_SPT1];
-#pragma unroll
-    for (int j = 0; j < EXPAND_SPT1; ++j) nsucc[j] = 0;
-    GroupRunner<0>::run(p, first, tile_base, count, spt, nsucc, failed, wbuf, wcnt);
-    flush_stage(p, wbuf, wcnt, true, failed);
-#pragma unroll
-    for (int j = 0; j < EXPAND_SPT1; ++j) {
-      uint64_t i = tile_base + (uint64_t)j * EXPAND_BLOCK + threadIdx.x;
-      if (j >= spt || i >= count) continue;
-      gen += nsucc[j];
-      if (nsucc[j] > maxfan) maxfan = nsucc[j];
-      if (nsucc[j] == 0) {
-        ++dead;
-        if (p.check_deadlock) {
-          State s;
-          load_state(s, p.store + ((first + i) & p.store_mask) * W);
-          record_violation(p, s, p.parent[(first + i) & p.store_mask], fingerprint(s), ~0ull);
-        }
-      }
-    }
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    gen += __shfl_xor_sync(0xffffffffu, gen, o);
-    dead += __shfl_xor_sync(0xffffffffu, dead, o);
-    maxfan = max(maxfan, __shfl_xor_sync(0xffffffffu, maxfan, o));
-    failed = max(failed, __shfl_xor_sync(0xffffffffu, failed, o));
-  }
-  if (lane_id() == 0) {
-    if (gen) atomicAdd(&p.ctr->generated, gen);
-    if (dead) atomicAdd(&p.ctr->deadlocks, dead);
-    if (maxfan) atomicMax(&p.ctr->max_fanout_seen, (unsigned long long)maxfan);
-    if (failed) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)failed);
-  }
-}
-#endif  // KMC_ONE_PHASE
 
 __device__ __forceinline__ void load_row(State& s, uint64_t& meta, const uint64_t* rows, uint64_t i, bool valid) {
   meta = 0;
@@ -1186,7 +1051,6 @@ struct Engine {
   bool timing = true;
   bool count_actions = false;
   uint64_t stop_after_states = 0;   // bounded run: stop at the first level end with >= this many states
-  int l2_fetch = 0;                 // cudaLimitMaxL2FetchGranularity hint (32/64/128), 0 = leave the default
   uint32_t fanout_bound = 0;        // successors per state assumed when sizing a frontier chunk (0: min(MAX_FANOUT, 32))
   // spill / checkpoint (single rank): the device store is a ring over the live window [store_base, tail); the
   // levels below the one being expanded move to host memory (TLC's DiskStateQueue / trace file on disk)
@@ -1196,13 +1060,6 @@ struct Engine {
   std::string checkpoint_dir, recover_dir;
   double checkpoint_minutes = 0;    // 0: a checkpoint after every level (when checkpoint_dir is set)
   std::chrono::steady_clock::time_point last_checkpoint;
-  bool overlap = false;             // single rank: K2 of chunk i runs on a second stream while K1 expands chunk i+1
-                                    // (K1 is issue-bound, K2 waits on random DRAM sectors: they use different units)
-  cudaStream_t stream2 = nullptr;
-  cudaEvent_t ev_exp[2] = {nullptr, nullptr}, ev_ins[2] = {nullptr, nullptr};
-  bool prefetch = false;            // K1 prefetches candidate buckets into L2 (pair with a small chunk_states)
-  uint64_t chunk_states_opt = 0;    // frontier states per K1/K2 launch pair (0: as many as the candidate buffer allows)
-  bool one_phase = false;           // comparison only: the round-1 one-phase K1 (needs a -DKMC_ONE_PHASE build)
 
   void* table = nullptr;
   uint64_t table_slots = 0;             // slots of SLOT_BYTES each
@@ -1266,8 +1123,6 @@ struct Engine {
     p.world = world;
     p.check_deadlock = check_deadlock ? 1 : 0;
     p.count_actions = count_actions ? 1 : 0;
-    p.prefetch = prefetch ? 1 : 0;
-    p.cand_slot = 0;
     for (int r = 0; r < MAX_WORLD; ++r) p.peer_inbox[r] = peer_inbox[r];
     p.inbox_stride = inbox_stride;
     p.p2p = 0;
@@ -1345,18 +1200,17 @@ static cudaEvent_t get_event(Engine& E) {
 struct TimedLaunch {
   Engine& E;
   int kind;
-  cudaStream_t on;
   cudaEvent_t a = nullptr, b = nullptr;
-  TimedLaunch(Engine& e, int k, cudaStream_t s = nullptr) : E(e), kind(k), on(s ? s : e.stream) {
+  TimedLaunch(Engine& e, int k) : E(e), kind(k) {
     if (E.timing) {
       a = get_event(E);
       b = get_event(E);
-      cudaEventRecord(a, on);
+      cudaEventRecord(a, E.stream);
     }
   }
   ~TimedLaunch() {
     if (E.timing) {
-      cudaEventRecord(b, on);
+      cudaEventRecord(b, E.stream);
       E.launches.push_back({kind, a, b});
     }
   }
@@ -1384,7 +1238,6 @@ static int engine_alloc(Engine& E) {
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, E.device));
   E.sms = prop.multiProcessorCount;
-  if (E.l2_fetch) CK(cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)E.l2_fetch));
   size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
   // Default sizing from the memory that is actually free: candidate buffers first, then set + store + parent
@@ -1419,9 +1272,7 @@ static int engine_alloc(Engine& E) {
       E.max_states = p2;
     }
   }
-  uint64_t rows_total = E.cand_bytes / (ROW * 8);
-  if (E.world > 1) E.overlap = false;                    // (the fused exchange double-buffers on its own)
-  E.region_rows = rows_total / (E.overlap ? 2 : E.world);
+  E.region_rows = E.cand_bytes / (ROW * 8) / E.world;
   if (E.region_rows < (uint64_t)M::MAX_FANOUT) E.region_rows = M::MAX_FANOUT;
   // A chunk of frontier states is sized for `fanout_bound` successors per state on average *per owner region*.
   // MAX_FANOUT (emit sites in expand) is a safe but very loose bound -- reachable states enable a small
@@ -1429,19 +1280,11 @@ static int engine_alloc(Engine& E) {
   // assumes <= 32 and relies on the kernel's overflow check (KMC_E_CAND_FULL, nothing is lost silently).
   if (E.fanout_bound == 0) E.fanout_bound = std::min<uint32_t>((uint32_t)M::MAX_FANOUT, 32u);
   E.chunk_states = std::max<uint64_t>(1, E.region_rows / E.fanout_bound);
-  if (E.chunk_states_opt) E.chunk_states = std::min<uint64_t>(E.chunk_states, E.chunk_states_opt);
   if (E.own_stream) CK(cudaStreamCreateWithFlags(&E.stream, cudaStreamNonBlocking));
-  if (E.overlap) {
-    CK(cudaStreamCreateWithFlags(&E.stream2, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-      CK(cudaEventCreateWithFlags(&E.ev_exp[i], cudaEventDisableTiming));
-      CK(cudaEventCreateWithFlags(&E.ev_ins[i], cudaEventDisableTiming));
-    }
-  }
   CK(cudaMalloc(&E.table, E.table_slots * SLOT_BYTES));
   CK(cudaMalloc(&E.store, E.max_states * W * 8));
   CK(cudaMalloc(&E.parent, E.max_states * 8));
-  CK(cudaMalloc(&E.cand, E.region_rows * (E.overlap ? 2 : E.world) * ROW * 8));
+  CK(cudaMalloc(&E.cand, E.region_rows * E.world * ROW * 8));
   if (E.world > 1) {
     E.recv_rows = E.region_rows * E.world;
     CK(cudaMalloc(&E.recv, E.recv_rows * ROW * 8));
@@ -1454,14 +1297,6 @@ static int engine_alloc(Engine& E) {
   }
   // the expand kernel keeps its state tile, the successor stage and the pair list in > 48 KB of dynamic shared memory
   CK(cudaFuncSetAttribute(k_expand, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EXPAND_SMEM_BYTES));
-#ifdef KMC_ONE_PHASE
-  CK(cudaFuncSetAttribute(k_expand1, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGE_BYTES + NWARPS * 4));
-#else
-  if (E.one_phase) {
-    E.last_error = "option one_phase needs a library built with -DKMC_ONE_PHASE";
-    return KMC_E_BADARG;
-  }
-#endif
   CK(cudaMalloc(&E.ctr, sizeof(DevCounters)));
   CK(cudaMalloc(&E.viol_ring, (size_t)VIOL_RING * VIOL_ROW * 8));
   CK(cudaEventCreate(&E.ev_begin));
@@ -1538,11 +1373,11 @@ static int seed_init(Engine& E) {
 }
 
 static int launch_insert(Engine& E, const uint64_t* rows, const unsigned long long* n_dev, uint64_t n_fixed,
-                         uint64_t n_bound, cudaStream_t on = nullptr) {
+                         uint64_t n_bound) {
   Params p = E.params();
   {
-    TimedLaunch t(E, 1, on);
-    k_insert<<<grid_for(E, n_bound, 256, 8), 256, 0, on ? on : E.stream>>>(p, rows, n_dev, n_fixed);
+    TimedLaunch t(E, 1);
+    k_insert<<<grid_for(E, n_bound, 256, 8), 256, 0, E.stream>>>(p, rows, n_dev, n_fixed);
   }
   CK(cudaGetLastError());
   return KMC_OK;
@@ -1557,26 +1392,13 @@ static int launch_invariants(Engine& E, uint64_t first, uint64_t count_bound) {
   return KMC_OK;
 }
 
-static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false, uint32_t slot = 0) {
+static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false) {
   Params p = E.params();
   p.p2p = p2p ? 1 : 0;
-  p.cand_slot = slot;
-  p.cand = E.cand + (uint64_t)slot * E.region_rows * ROW;
   if (count == 0) return KMC_OK;
   TimedLaunch t(E, 0);
-#ifdef KMC_ONE_PHASE
-  if (E.one_phase) {
-    int spt = EXPAND_SPT1;
-    while (spt > 1 && count < (uint64_t)E.sms * EXPAND_BLOCK * spt) spt >>= 1;
-    uint64_t tiles = (count + (uint64_t)EXPAND_BLOCK * spt - 1) / ((uint64_t)EXPAND_BLOCK * spt);
-    int grid = (int)std::min<uint64_t>(std::max<uint64_t>(tiles, 1), (uint64_t)E.sms);
-    k_expand1<<<grid, EXPAND_BLOCK, STAGE_BYTES + NWARPS * 4, E.stream>>>(p, first, count, spt);
-    CK(cudaGetLastError());
-    return KMC_OK;
-  }
-#endif
   // small levels: smaller tiles so that every SM still gets one (a tile is a multiple of 32 states)
-  const uint64_t ctas = (uint64_t)E.sms * EXPAND_CTAS_PER_SM;
+  const uint64_t ctas = (uint64_t)E.sms;
   uint64_t per_cta = (count + ctas - 1) / ctas;
   unsigned tile_states = (unsigned)std::min<uint64_t>((uint64_t)TILE, std::max<uint64_t>(32, (per_cta + 31) & ~31ull));
   uint64_t tiles = (count + tile_states - 1) / tile_states;
@@ -1857,35 +1679,13 @@ static int engine_run(Engine& E) {
   while (!err && !stopped && level_end > level_first) {
     E.widths.push_back(level_end - level_first);
     if ((rc = spill_below(E, level_first))) return rc;         // (no-op unless spilling)
-    // a chunk never crosses the wrap of the ring store
-    auto chunk_len = [&](uint64_t off) {
-      uint64_t cnt = std::min<uint64_t>(E.chunk_states, level_end - off);
+    for (uint64_t off = level_first, cnt; off < level_end; off += cnt) {
+      cnt = std::min<uint64_t>(E.chunk_states, level_end - off);
+      // a chunk never crosses the wrap of the ring store
       if (E.spill) cnt = std::min<uint64_t>(cnt, E.max_states - (off & (E.max_states - 1)));
-      return cnt;
-    };
-    if (E.overlap) {
-      // K1 of chunk i+1 (stream) overlaps K2 of chunk i (stream2); the two halves of the candidate buffer alternate
-      uint32_t slot = 0;
-      for (uint64_t off = level_first, cnt; off < level_end; off += cnt, slot ^= 1) {
-        cnt = chunk_len(off);
-        CK(cudaStreamWaitEvent(E.stream, E.ev_ins[slot], 0));            // the K2 that read this half has finished
-        CK(cudaMemsetAsync(&E.ctr->cand_count[slot], 0, sizeof(unsigned long long), E.stream));
-        if ((rc = launch_expand(E, off, cnt, false, slot))) return rc;
-        CK(cudaEventRecord(E.ev_exp[slot], E.stream));
-        CK(cudaStreamWaitEvent(E.stream2, E.ev_exp[slot], 0));
-        if ((rc = launch_insert(E, E.cand + (uint64_t)slot * E.region_rows * ROW, &E.ctr->cand_count[slot], 0,
-                                cnt * (uint64_t)E.fanout_bound, E.stream2))) return rc;
-        CK(cudaEventRecord(E.ev_ins[slot], E.stream2));
-      }
-      CK(cudaStreamWaitEvent(E.stream, E.ev_ins[0], 0));
-      CK(cudaStreamWaitEvent(E.stream, E.ev_ins[1], 0));
-    } else {
-      for (uint64_t off = level_first, cnt; off < level_end; off += cnt) {
-        cnt = chunk_len(off);
-        if ((rc = reset_cand(E))) return rc;
-        if ((rc = launch_expand(E, off, cnt))) return rc;
-        if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, cnt * (uint64_t)E.fanout_bound))) return rc;
-      }
+      if ((rc = reset_cand(E))) return rc;
+      if ((rc = launch_expand(E, off, cnt))) return rc;
+      if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, cnt * (uint64_t)E.fanout_bound))) return rc;
     }
     if ((rc = launch_invariants(E, level_end, (level_end - level_first) * 2))) return rc;
     if ((rc = read_counters(E, &h))) return rc;
@@ -1975,15 +1775,10 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
   if (json_bool(options_json, "timing", &b)) E.timing = b;
   if (json_bool(options_json, "count_actions", &b)) E.count_actions = b;
   if (json_num(options_json, "stop_after_states", &d)) E.stop_after_states = (uint64_t)d;
-  if (json_num(options_json, "l2_fetch", &d)) E.l2_fetch = (int)d;
-  if (json_bool(options_json, "one_phase", &b)) E.one_phase = b;
-  if (json_bool(options_json, "prefetch", &b)) E.prefetch = b;
-  if (json_bool(options_json, "overlap", &b)) E.overlap = b;
   if (json_bool(options_json, "spill", &b)) E.spill = b;
   json_str(options_json, "checkpoint_dir", &E.checkpoint_dir);
   json_str(options_json, "recover", &E.recover_dir);
   if (json_num(options_json, "checkpoint_minutes", &d)) E.checkpoint_minutes = d;
-  if (json_num(options_json, "chunk_states", &d)) E.chunk_states_opt = (uint64_t)d;
   if (json_num(options_json, "fanout_bound", &d)) E.fanout_bound = (uint32_t)d;
   if (json_num(options_json, "stream", &d) && d != 0) {
     // a cudaStream_t handle of the calling process (e.g. torch.cuda.current_stream().cuda_stream): engine
@@ -2029,11 +1824,6 @@ void kmcm_destroy(kmcm_ctx* c) {
   if (E.ev_begin) cudaEventDestroy(E.ev_begin);
   if (E.ev_end) cudaEventDestroy(E.ev_end);
   if (E.stream && E.own_stream) cudaStreamDestroy(E.stream);
-  if (E.stream2) cudaStreamDestroy(E.stream2);
-  for (int i = 0; i < 2; ++i) {
-    if (E.ev_exp[i]) cudaEventDestroy(E.ev_exp[i]);
-    if (E.ev_ins[i]) cudaEventDestroy(E.ev_ins[i]);
-  }
   delete c;
 }
 

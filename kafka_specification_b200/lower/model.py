@@ -524,8 +524,12 @@ struct State {{ uint64_t w[W]; }};
 """
 
 
-def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | None = None,
-                group_lines: int = 160, max_group_sites: int = 64, guard_lines: int = 3000) -> LoweredModel:
+GROUP_LINES = 160         # one-phase form: lines of Next per expand_group
+MAX_GROUP_SITES = 64      # two-phase form: emit sites per site group (one 64-bit mask word)
+GUARD_LINES = 3000        # two-phase form: a site group closes once its guard code is longer than this
+
+
+def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | None = None) -> LoweredModel:
     cfg = parse_cfg(cfg_text)
     root = load_root(module, search_dirs)
     lw = Lowerer(root, cfg)
@@ -610,10 +614,9 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     lw.gen_next(start, {}, None)
     lw.end_unit()
     expand_prologue = list(lw.prologue)
-    # One-phase form: pack consecutive units into groups of bounded size: each group becomes one function that
-    # is swept over a tile of states, so that its code stays resident in the SM's instruction cache (a fully
-    # unrolled Next is hundreds of KB of SASS).  Kept for the host-side harness / CPU baseline and as the
-    # engine's -DKMC_ONE_PHASE comparison build.
+    # One-phase form: consecutive units packed into groups of bounded size, one function each; expand() calls them
+    # in order.  The host tests, the CPU baseline and the host-side shard stand-ins run it; the CUDA build skips
+    # this section of the header (-DKMC_NO_ONE_PHASE) to keep nvcc time down.
     groups: list[list[str]] = []
     cur_lines: list[str] = []
     all_units: list[list[str]] = []
@@ -621,7 +624,7 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
         top_blocks = sum(1 for n in _prune(_parse_unit(lines)) if n.is_block)
         all_units.extend(_split_unit(lines, 40) if top_blocks > 40 else [lines])
     for lines in all_units:
-        if cur_lines and len(cur_lines) + len(lines) > group_lines:
+        if cur_lines and len(cur_lines) + len(lines) > GROUP_LINES:
             groups.append(cur_lines)
             cur_lines = []
         cur_lines = cur_lines + ["  {"] + ["  " + l for l in lines] + ["  }"]
@@ -639,8 +642,8 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     for tree, sites in unit_trees:
         k = 0
         while k < len(sites):
-            room = max_group_sites - cur["count"]
-            if room == 0 or (cur["count"] and len(cur["guard"]) > guard_lines):
+            room = MAX_GROUP_SITES - cur["count"]
+            if room == 0 or (cur["count"] and len(cur["guard"]) > GUARD_LINES):
                 site_groups.append(cur)
                 cur = {"begin": cur["begin"] + cur["count"], "count": 0, "guard": []}
                 continue
