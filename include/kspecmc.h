@@ -17,6 +17,8 @@
  *   kmc_stats           ModelChecker.reportSuccess / printSummary ("N states generated,
  *                       M distinct states found, Q states left on queue", depth)
  *   kmc_violation       ModelChecker.doNext's invariant/deadlock failure report
+ *   kmc_coverage        ModelChecker's coverage report (TLC -coverage: "distinct:generated" per action, at the
+ *                       action level of TLC >= 1.7), from counters the kernels keep on every run
  *   kmc_trace_*         tlc2.tool.TLCTrace.getTrace / printTrace (error trace by parent links)
  *   kmc_fpset_*         tlc2.tool.fp.FPSet.put / contains / size (the set alone, for callers
  *                       that keep TLC's own Worker loop)
@@ -115,8 +117,9 @@ typedef struct {
  * "spill":false (the state store is a ring over the live BFS window, max_states slots rounded down to a power of
  *   two; older levels move to host memory -- TLC's DiskStateQueue),
  * "checkpoint_dir":"d", "checkpoint_minutes":M (TLC -checkpoint: states + parent links + counters written at a level
- *   boundary at most every M minutes, 0 = every level), "recover":"d" (TLC -recover: continue from that checkpoint;
- *   the set is rebuilt from the stored states).  */
+ *   boundary at most every M minutes, 0 = every level; the per-site coverage counts are part of it),
+ *   "recover":"d" (TLC -recover: continue from that checkpoint; the set is rebuilt from the stored states).
+ * Unknown keys are ignored.  */
 int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out);
 void kmc_destroy(kmc_ctx* ctx);
 int kmc_model_info(const kmc_ctx* ctx, kmc_model_info_t* out);
@@ -124,7 +127,21 @@ int kmc_model_info(const kmc_ctx* ctx, kmc_model_info_t* out);
 int kmc_run(kmc_ctx* ctx);                                   /* blocking full BFS         */
 int kmc_stats(const kmc_ctx* ctx, kmc_stats_t* out);
 int kmc_level_widths(const kmc_ctx* ctx, uint64_t* out, size_t cap, size_t* n);
+/* successors generated per action of the last run (index = action id of the parent words); *n = number of actions */
 int kmc_action_counts(const kmc_ctx* ctx, uint64_t* out, size_t cap, size_t* n);
+/* Coverage of the last run (TLC -coverage), kept by the kernels on every run at no measurable cost:
+ *   action_generated[a]  successors produced by action a (duplicates and successors a CONSTRAINT discards included)
+ *   action_distinct[a]   new states whose parent word carries action a (initial states are not counted)
+ *   site_generated[i]    successors produced by emit site i of the lowered Next (model.json "sites" maps i to its action)
+ * Up to action_cap / site_cap entries are written; *n_actions / *n_sites receive the full counts.  Generated per action
+ * is deterministic, and so is generated per site without SYMMETRY (with it, the orbit member that is stored and
+ * expanded is the one whose insert won, and members spread their successors differently over per-replica sites).
+ * Distinct per action depends on which generator of a new state won the insert (as in TLC with more than one
+ * worker), and sum(distinct) + initial states = distinct states.  *complete = 0 after recovering from a
+ * checkpoint written without per-site counts: the generated counts then cover only the levels run since.  With
+ * "gpus": N the counts are summed over the GPUs; a multi-process (kmc_shard_*) driver reads them per rank. */
+int kmc_coverage(const kmc_ctx* ctx, uint64_t* action_generated, uint64_t* action_distinct, size_t action_cap,
+                 uint64_t* site_generated, size_t site_cap, size_t* n_actions, size_t* n_sites, int32_t* complete);
 int kmc_violation(const kmc_ctx* ctx, kmc_violation_t* out);
 /* i-th state of the error trace (0 = an initial state); buf receives `words` uint64_t.    */
 int kmc_trace_state(const kmc_ctx* ctx, uint32_t i, uint64_t* buf, size_t cap_words, uint32_t* action_id);

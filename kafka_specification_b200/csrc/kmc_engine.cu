@@ -165,7 +165,9 @@ struct DevCounters {
   unsigned long long fail;
   unsigned long long max_fanout_seen;
   unsigned long long viol_count;         // rows claimed in the violator ring
-  unsigned long long action_counts[64];
+  // coverage (TLC -coverage), kept over all levels of a run:
+  unsigned long long site_generated[M::NUM_SITES > 0 ? M::NUM_SITES : 1];   // successors per emit site (K1's A1 totals)
+  unsigned long long action_distinct[M::NUM_ACTIONS];   // new states per action (K2, from the winners' parent words)
 };
 
 // Violating states are rare and terminal, so they go to a small ring: W state words, the
@@ -189,7 +191,6 @@ struct Params {
   uint64_t* viol_ring;
   uint32_t rank, world;
   uint32_t check_deadlock;
-  uint32_t count_actions;
   // fused exchange (world > 1, after kmc_shard_open_peers): every rank's inbox, mapped into this
   // process through CUDA IPC.  An inbox is two buffers (double buffering); a buffer is an 8-word
   // header (rows sent by each source rank) followed by world regions of region_rows rows.
@@ -375,6 +376,12 @@ __device__ __forceinline__ void insert_row(const Params& p, const State& s, uint
     if ((int)lane == leader) base = atomicAdd(&p.ctr->store_tail, (unsigned long long)__popc(mask));
     base = __shfl_sync(0xffffffffu, base, leader);
     if (is_new) {
+      // coverage: distinct states per action = the action bits of the winners' parent words (initial states have
+      // none); one atomic per action present among the warp's winners
+      const unsigned act = ((meta & 0x0000FFFFFFFFFFFFull) == NO_PARENT) ? ~0u : (unsigned)(meta >> 56);
+      const unsigned same = __match_any_sync(mask, act);
+      if (act < (unsigned)M::NUM_ACTIONS && (int)lane == __ffs(same) - 1)
+        atomicAdd(&p.ctr->action_distinct[act], (unsigned long long)__popc(same));
       uint64_t idx = base + __popc(mask & ((1u << lane) - 1));
       if (idx - p.store_base < p.max_states) {
         uint64_t* dst = p.store + (idx & p.store_mask) * W;
@@ -483,7 +490,6 @@ struct CandSink {
   uint64_t parent_ref;
   uint32_t wbuf;       // this warp's staging rows (shared-window address)
   uint32_t wcnt;       // rows staged by this warp (shared-window address)
-  unsigned long long* action_counts;   // per-action counters (global memory), or nullptr
   int n;
   int failed;
 
@@ -506,7 +512,6 @@ struct CandSink {
       // cannot happen (a body pass adds <= 32 rows to a stage that is flushed at >= STAGE_FLUSH)
       failed = KMC_FAIL_CAND_FULL;
     }
-    if (action_counts != nullptr && action < 64) atomicAdd(action_counts + action, 1ull);
   }
   __device__ __forceinline__ void fail(int code) { failed = code; }
 };
@@ -530,7 +535,9 @@ __device__ __forceinline__ void load_state(State& s, const uint64_t* src) {
 //   B   the list is consumed 32 entries at a time; a chunk belongs to exactly one site, so the body
 //       dispatch is warp-uniform and the body runs with (almost) all lanes on the same code.
 //       B of group g overlaps A1 of group g+1 (double-buffered totals): two barriers per group.
-// Successor counts per state (deadlock detection, "states generated") are popc(mask).
+// Successor counts per state (deadlock detection, "states generated") are popc(mask).  The A1 totals are also the
+// coverage counts: each CTA adds them up per emit site in shared memory and flushes them with one global atomic per
+// site at the end of the kernel.
 // ----------------------------------------------------------------------------------------
 static constexpr int STAGE_BYTES = NWARPS * STAGE_ROWS * ROW * 8;
 static constexpr int FIXED_SMEM_BYTES = STAGE_BYTES + LIST_CAP * 2 + (4 * MAX_GROUP_SITES + NWARPS + 8) * 4;
@@ -539,7 +546,10 @@ static constexpr int SPT = SPT_FIT > 4 ? 4 : SPT_FIT;
 static_assert(SPT >= 1, "state too wide for the expand kernel's shared-memory tile");
 static constexpr int TILE = EXPAND_BLOCK * SPT;
 static_assert(TILE <= LIST_CAP, "a site's segment (<= TILE pairs) must fit one scatter round");
-static constexpr size_t EXPAND_SMEM_BYTES = (size_t)TILE * W * 8 + FIXED_SMEM_BYTES;
+// the per-site coverage counters live in the slack the tile leaves (SPT is sized without them)
+static constexpr int SITE_GEN_BYTES = (M::NUM_SITES > 0 ? M::NUM_SITES : 1) * 8;
+static constexpr size_t EXPAND_SMEM_BYTES = (size_t)TILE * W * 8 + FIXED_SMEM_BYTES + SITE_GEN_BYTES;
+static_assert(EXPAND_SMEM_BYTES <= 227 * 1024 - 1024, "the per-site coverage counters do not fit next to the expand tile");
 
 struct TileCtx {
   uint32_t tile;        // [TILE][W] states (shared-window addresses throughout)
@@ -547,6 +557,7 @@ struct TileCtx {
   uint32_t cnt;         // [2][MAX_GROUP_SITES] enabled pairs per site (double-buffered across groups)
   uint32_t cur;         // [MAX_GROUP_SITES] scatter cursors
   uint32_t seg;         // [MAX_GROUP_SITES] first chunk of each site's segment
+  uint32_t site_gen;    // [NUM_SITES] u64: successors this CTA generated per emit site
   uint32_t wbuf, wcnt;
   uint64_t first, tile_base;
   unsigned nvalid;      // states in this tile
@@ -620,6 +631,11 @@ struct SiteGroupRunner {
       }
     }
     __syncthreads();                                   // totals complete; B of the previous group finished
+    // coverage: thread k adds this tile's total of site BEGIN + k (no other thread touches that counter)
+    if (threadIdx.x < (unsigned)NS) {
+      const uint32_t a = c.site_gen + (BEGIN + threadIdx.x) * 8;
+      sts64(a, lds64(a) + lds32(cnt + threadIdx.x * 4));
+    }
     // the other totals buffer (read last by B of group G-1) is cleared for A1 of group G+1
     if (threadIdx.x < MAX_GROUP_SITES) sts32(c.cnt + ((G + 1) & 1) * (MAX_GROUP_SITES * 4) + threadIdx.x * 4, 0u);
     // ---- every warp: the same padded segment layout, sites 2*lane and 2*lane+1 per lane
@@ -699,8 +715,7 @@ struct SiteGroupRunner {
           State s;
 #pragma unroll
           for (int q = 0; q < W; ++q) s.w[q] = lds64(c.tile + (slot * W + q) * 8);
-          CandSink sink{(c.first + c.tile_base + slot) | ((uint64_t)p.rank << 40), c.wbuf, c.wcnt,
-                        p.count_actions ? p.ctr->action_counts : nullptr, 0, 0};
+          CandSink sink{(c.first + c.tile_base + slot) | ((uint64_t)p.rank << 40), c.wbuf, c.wcnt, 0, 0};
           SiteDispatch<BEGIN, END>::run(k + BEGIN, s, sink);
           failed |= sink.failed;
         }
@@ -717,7 +732,7 @@ struct SiteGroupRunner<M::NUM_SITE_GROUPS> {
 };
 
 __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t first, uint64_t count, unsigned tile_states) {
-  extern __shared__ __align__(16) uint64_t smem[];   // tile | stage | list | cnt[2][64] | cur[64] | seg[64] | wcnt[NWARPS]
+  extern __shared__ __align__(16) uint64_t smem[];   // tile | stage | list | cnt[2][64] | cur[64] | seg[64] | wcnt[NWARPS] | - | site_gen
   const int warp = threadIdx.x >> 5;
   TileCtx c;
   c.tile = smem_addr(smem);
@@ -728,8 +743,10 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
   c.cur = c.cnt + 2 * MAX_GROUP_SITES * 4;
   c.seg = c.cur + MAX_GROUP_SITES * 4;
   c.wcnt = c.seg + MAX_GROUP_SITES * 4 + warp * 4;
+  c.site_gen = c.seg + MAX_GROUP_SITES * 4 + (NWARPS + 8) * 4;
   c.first = first;
   if (lane_id() == 0) sts32(c.wcnt, 0u);
+  for (unsigned i = threadIdx.x; i < (unsigned)M::NUM_SITES; i += EXPAND_BLOCK) sts64(c.site_gen + i * 8, 0ull);
   unsigned long long gen = 0, dead = 0;
   unsigned maxfan = 0;
   int failed = 0;
@@ -776,6 +793,12 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
         }
       }
     }
+  }
+  // coverage: one atomic per (CTA, site)
+  __syncthreads();
+  for (unsigned i = threadIdx.x; i < (unsigned)M::NUM_SITES; i += EXPAND_BLOCK) {
+    const unsigned long long v = lds64(c.site_gen + i * 8);
+    if (v) atomicAdd(&p.ctr->site_generated[i], v);
   }
   // warp reduce the statistics, one atomic per warp
   for (int o = 16; o > 0; o >>= 1) {
@@ -1049,7 +1072,6 @@ struct Engine {
   bool cont = false;
   bool check_deadlock = M::CHECK_DEADLOCK;
   bool timing = true;
-  bool count_actions = false;
   uint64_t stop_after_states = 0;   // bounded run: stop at the first level end with >= this many states
   uint32_t fanout_bound = 0;        // successors per state assumed when sizing a frontier chunk (0: min(MAX_FANOUT, 32))
   // spill / checkpoint (single rank): the device store is a ring over the live window [store_base, tail); the
@@ -1095,7 +1117,11 @@ struct Engine {
   mutable std::mutex mu;
   kmc_stats_t stats{};
   std::vector<uint64_t> widths;
-  std::vector<uint64_t> action_counts;
+  // coverage of the last run (host copies of the device counters, summed over the ranks of a "gpus" context);
+  // incomplete after recovering from a checkpoint that predates the per-site counts
+  std::vector<uint64_t> site_generated = std::vector<uint64_t>(M::NUM_SITES, 0);
+  std::vector<uint64_t> action_distinct = std::vector<uint64_t>(M::NUM_ACTIONS, 0);
+  bool coverage_complete = true;
   kmc_violation_t viol{};
   std::vector<std::vector<uint64_t>> trace;
   std::vector<uint32_t> trace_actions;
@@ -1122,7 +1148,6 @@ struct Engine {
     p.rank = rank;
     p.world = world;
     p.check_deadlock = check_deadlock ? 1 : 0;
-    p.count_actions = count_actions ? 1 : 0;
     for (int r = 0; r < MAX_WORLD; ++r) p.peer_inbox[r] = peer_inbox[r];
     p.inbox_stride = inbox_stride;
     p.p2p = 0;
@@ -1323,7 +1348,20 @@ static int engine_reset(Engine& E) {
   E.store_base = 0;
   E.host_store.clear();
   E.host_parent.clear();
+  {
+    std::lock_guard<std::mutex> g(E.mu);
+    std::fill(E.site_generated.begin(), E.site_generated.end(), 0);
+    std::fill(E.action_distinct.begin(), E.action_distinct.end(), 0);
+    E.coverage_complete = true;
+  }
   return KMC_OK;
+}
+
+// host copy of the coverage counters (the caller has just read them from the device)
+static void keep_coverage(Engine& E, const DevCounters& h) {
+  std::lock_guard<std::mutex> g(E.mu);
+  E.site_generated.assign(h.site_generated, h.site_generated + M::NUM_SITES);
+  E.action_distinct.assign(h.action_distinct, h.action_distinct + M::NUM_ACTIONS);
 }
 
 static int read_counters(Engine& E, DevCounters* h) {
@@ -1482,10 +1520,14 @@ static int write_checkpoint(Engine& E, const DevCounters& h, const LevelCursor& 
   f = fopen((meta + ".tmp").c_str(), "w");
   if (!f) return KMC_E_BADARG;
   fprintf(f, "model %s\ndigest %s\nwords %d\ntail %llu\nlevel_first %llu\nlevel_end %llu\nlevel %llu\ngenerated %llu\n"
-             "deadlocks %llu\nout_of_model %llu\nprobes %llu\nwidths",
+             "deadlocks %llu\nout_of_model %llu\nprobes %llu\nsite_generated",
           KMC_MODEL_NAME, KMC_MODEL_DIGEST, W, (unsigned long long)tail, (unsigned long long)lc.level_first,
           (unsigned long long)lc.level_end, (unsigned long long)lc.level, (unsigned long long)h.generated,
           (unsigned long long)h.deadlocks, (unsigned long long)h.out_of_model, (unsigned long long)h.probes);
+  // (before widths: a reader stops at widths.  Distinct per action is not written: it is the histogram of the
+  // parent words, which recover reads anyway)
+  for (int i = 0; i < M::NUM_SITES; ++i) fprintf(f, " %llu", (unsigned long long)h.site_generated[i]);
+  fprintf(f, "\nwidths");
   for (uint64_t w : E.widths) fprintf(f, " %llu", (unsigned long long)w);
   fprintf(f, "\n");
   fclose(f);
@@ -1504,6 +1546,7 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
   char key[64], val[256];
   unsigned long long tail = 0, words = 0;
   std::string digest;
+  bool have_sites = false;
   memset(h, 0, sizeof(*h));
   E.widths.clear();
   while (fscanf(f, "%63s", key) == 1) {
@@ -1511,6 +1554,12 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
       unsigned long long w;
       while (fscanf(f, "%llu", &w) == 1) E.widths.push_back(w);
       break;
+    }
+    if (!strcmp(key, "site_generated")) {
+      int i = 0;
+      for (; i < M::NUM_SITES && fscanf(f, "%llu", &h->site_generated[i]) == 1; ++i) {}
+      have_sites = i == M::NUM_SITES;
+      continue;
     }
     if (fscanf(f, "%255s", val) != 1) break;
     const unsigned long long v = strtoull(val, nullptr, 10);
@@ -1549,6 +1598,14 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
     E.last_error = "short read on " + bin;
     return KMC_E_BADARG;
   }
+  // distinct per action: the action bits of the stored parent words (initial states have none)
+  for (uint64_t g = 0; g < tail; ++g) {
+    if ((pa[g] & 0x0000FFFFFFFFFFFFull) == NO_PARENT) continue;
+    const uint64_t a = pa[g] >> 56;
+    if (a < (uint64_t)M::NUM_ACTIONS) h->action_distinct[a]++;
+  }
+  if (!have_sites) memset(h->site_generated, 0, sizeof(h->site_generated));
+  E.coverage_complete = have_sites;      // a checkpoint written before the per-site counts existed: generated is partial
   E.store_base = keep_from;
   E.host_store.assign(st.begin(), st.begin() + (size_t)keep_from * W);
   E.host_parent.assign(pa.begin(), pa.begin() + (size_t)keep_from);
@@ -1574,6 +1631,8 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
   CK(cudaMemcpyAsync(&E.ctr->deadlocks, &h->deadlocks, 8, cudaMemcpyHostToDevice, E.stream));
   CK(cudaMemcpyAsync(&E.ctr->out_of_model, &h->out_of_model, 8, cudaMemcpyHostToDevice, E.stream));
   CK(cudaMemcpyAsync(&E.ctr->probes, &h->probes, 8, cudaMemcpyHostToDevice, E.stream));
+  CK(cudaMemcpyAsync(E.ctr->site_generated, h->site_generated, sizeof(h->site_generated), cudaMemcpyHostToDevice, E.stream));
+  CK(cudaMemcpyAsync(E.ctr->action_distinct, h->action_distinct, sizeof(h->action_distinct), cudaMemcpyHostToDevice, E.stream));
   CK(cudaStreamSynchronize(E.stream));
   DevCounters now;
   int rc = read_counters(E, &now);
@@ -1744,9 +1803,9 @@ static int engine_run(Engine& E) {
     st.max_states = E.max_states;
     st.complete = (!err && !stopped) ? 1 : 0;
     if (E.timing) accumulate_timing(E, st);
-    E.action_counts.assign(h.action_counts, h.action_counts + 64);
     E.ran = true;
   }
+  keep_coverage(E, h);
   return err;
 }
 
@@ -1773,7 +1832,6 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
   if (json_bool(options_json, "continue", &b)) E.cont = b;
   if (json_bool(options_json, "check_deadlock", &b)) E.check_deadlock = b;
   if (json_bool(options_json, "timing", &b)) E.timing = b;
-  if (json_bool(options_json, "count_actions", &b)) E.count_actions = b;
   if (json_num(options_json, "stop_after_states", &d)) E.stop_after_states = (uint64_t)d;
   if (json_bool(options_json, "spill", &b)) E.spill = b;
   json_str(options_json, "checkpoint_dir", &E.checkpoint_dir);
@@ -1864,11 +1922,37 @@ int kmcm_level_widths(const kmcm_ctx* c, uint64_t* out, size_t cap, size_t* n) {
   return KMC_OK;
 }
 
+// generated per action = the per-site counts summed by the site's action
+static std::vector<uint64_t> action_generated(const Engine& e) {
+  std::vector<uint64_t> a(M::NUM_ACTIONS, 0);
+  for (int i = 0; i < M::NUM_SITES; ++i)
+    if (M::SITE_ACTION[i] >= 0 && M::SITE_ACTION[i] < M::NUM_ACTIONS) a[M::SITE_ACTION[i]] += e.site_generated[i];
+  return a;
+}
+
 int kmcm_action_counts(const kmcm_ctx* c, uint64_t* out, size_t cap, size_t* n) {
-  if (!c || !n) return KMC_E_BADARG;
+  if (!c || !n || (!out && cap)) return KMC_E_BADARG;
   std::lock_guard<std::mutex> g(E.mu);
-  *n = std::min<size_t>(M::NUM_ACTIONS, E.action_counts.size());
-  for (size_t i = 0; i < *n && i < cap; ++i) out[i] = E.action_counts[i];
+  const std::vector<uint64_t> a = action_generated(E);
+  *n = a.size();
+  for (size_t i = 0; i < a.size() && i < cap; ++i) out[i] = a[i];
+  return KMC_OK;
+}
+
+int kmcm_coverage(const kmcm_ctx* c, uint64_t* action_gen, uint64_t* action_dist, size_t action_cap, uint64_t* site_gen,
+                  size_t site_cap, size_t* n_actions, size_t* n_sites, int32_t* complete) {
+  if (!c || !n_actions || !n_sites || !complete) return KMC_E_BADARG;
+  if ((action_cap && (!action_gen || !action_dist)) || (site_cap && !site_gen)) return KMC_E_BADARG;
+  std::lock_guard<std::mutex> g(E.mu);
+  const std::vector<uint64_t> a = action_generated(E);
+  *n_actions = a.size();
+  *n_sites = E.site_generated.size();
+  *complete = E.coverage_complete ? 1 : 0;
+  for (size_t i = 0; i < a.size() && i < action_cap; ++i) {
+    action_gen[i] = a[i];
+    action_dist[i] = E.action_distinct[i];
+  }
+  for (size_t i = 0; i < E.site_generated.size() && i < site_cap; ++i) site_gen[i] = E.site_generated[i];
   return KMC_OK;
 }
 
@@ -2075,6 +2159,7 @@ int kmcm_shard_level_done(kmcm_ctx* c, uint64_t* level_first, uint64_t* level_co
     if (E.level_count) E.widths.push_back(E.level_count);
     E.stats.levels = E.stats.depth = E.widths.size();
   }
+  keep_coverage(E, h);
   if (h.viol_count && E.viol.kind == KMC_RESULT_OK) build_trace(E, h, E.shard_levels - 1);
   return fail_to_error(h.fail);
 }
@@ -2280,6 +2365,7 @@ int kmcm_shard_sync(kmcm_ctx* c) {
   {
     int rc = read_counters(E, &hc);              // synchronises the stream
     if (rc) return rc;
+    keep_coverage(E, hc);
     std::lock_guard<std::mutex> g(E.mu);
     E.stats.probes = hc.probes;
     E.stats.out_of_model = hc.out_of_model;
@@ -2433,6 +2519,14 @@ static int multi_run(kmcm_ctx* c) {
   }
   st.depth = st.levels = A.widths.size();
   st.complete = (!rc && !out[0].stopped) ? 1 : 0;
+  std::fill(A.site_generated.begin(), A.site_generated.end(), 0);
+  std::fill(A.action_distinct.begin(), A.action_distinct.end(), 0);
+  for (size_t r = 0; r < n; ++r) {
+    const Engine& R = c->ranks[r]->e;
+    std::lock_guard<std::mutex> gr(R.mu);
+    for (size_t i = 0; i < A.site_generated.size(); ++i) A.site_generated[i] += R.site_generated[i];
+    for (size_t i = 0; i < A.action_distinct.size(); ++i) A.action_distinct[i] += R.action_distinct[i];
+  }
   if (out[0].stopped && !rc) {
     // the states of the last level were inserted but not expanded: they are the queue
     for (size_t r = 0; r < n; ++r) st.queue += out[0].board[r * BOARD_WORDS + 1];

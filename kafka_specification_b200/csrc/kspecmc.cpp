@@ -27,6 +27,7 @@ struct kmc_ctx {
   int (*stats)(const kmcm_ctx*, kmc_stats_t*) = nullptr;
   int (*level_widths)(const kmcm_ctx*, uint64_t*, size_t, size_t*) = nullptr;
   int (*action_counts)(const kmcm_ctx*, uint64_t*, size_t, size_t*) = nullptr;
+  int (*coverage)(const kmcm_ctx*, uint64_t*, uint64_t*, size_t, uint64_t*, size_t, size_t*, size_t*, int32_t*) = nullptr;
   int (*violation)(const kmcm_ctx*, kmc_violation_t*) = nullptr;
   int (*trace_state)(const kmcm_ctx*, uint32_t, uint64_t*, size_t, uint32_t*) = nullptr;
   int (*copy_states)(const kmcm_ctx*, uint64_t, uint64_t, uint64_t*) = nullptr;
@@ -81,7 +82,8 @@ int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out) {
   bool ok = bind(c, c->create, "kmcm_create") && bind(c, c->destroy, "kmcm_destroy") &&
             bind(c, c->model_info, "kmcm_model_info") && bind(c, c->run, "kmcm_run") &&
             bind(c, c->stats, "kmcm_stats") && bind(c, c->level_widths, "kmcm_level_widths") &&
-            bind(c, c->action_counts, "kmcm_action_counts") && bind(c, c->violation, "kmcm_violation") &&
+            bind(c, c->action_counts, "kmcm_action_counts") && bind(c, c->coverage, "kmcm_coverage") &&
+            bind(c, c->violation, "kmcm_violation") &&
             bind(c, c->trace_state, "kmcm_trace_state") && bind(c, c->copy_states, "kmcm_copy_states") &&
             bind(c, c->copy_parents, "kmcm_copy_parents") && bind(c, c->violation_record, "kmcm_violation_record") &&
             bind(c, c->strerror_, "kmcm_strerror") && bind(c, c->fpset_put, "kmcm_fpset_put") &&
@@ -122,6 +124,10 @@ int kmc_run(kmc_ctx* c) { FWD(run); }
 int kmc_stats(const kmc_ctx* c, kmc_stats_t* out) { FWD(stats, out); }
 int kmc_level_widths(const kmc_ctx* c, uint64_t* out, size_t cap, size_t* n) { FWD(level_widths, out, cap, n); }
 int kmc_action_counts(const kmc_ctx* c, uint64_t* out, size_t cap, size_t* n) { FWD(action_counts, out, cap, n); }
+int kmc_coverage(const kmc_ctx* c, uint64_t* action_gen, uint64_t* action_dist, size_t action_cap, uint64_t* site_gen,
+                 size_t site_cap, size_t* n_actions, size_t* n_sites, int32_t* complete) {
+  FWD(coverage, action_gen, action_dist, action_cap, site_gen, site_cap, n_actions, n_sites, complete);
+}
 int kmc_violation(const kmc_ctx* c, kmc_violation_t* out) { FWD(violation, out); }
 int kmc_trace_state(const kmc_ctx* c, uint32_t i, uint64_t* buf, size_t cap, uint32_t* a) { FWD(trace_state, i, buf, cap, a); }
 int kmc_copy_states(const kmc_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) { FWD(copy_states, first, count, buf); }

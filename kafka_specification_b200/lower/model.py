@@ -11,6 +11,7 @@ from __future__ import annotations
 import copy
 import hashlib
 import json
+import re
 from dataclasses import dataclass, field
 
 from ..frontend.cfg import Config, ModelValue, parse_cfg
@@ -42,6 +43,9 @@ class LoweredModel:
     digest: str = ""
     lowerer: object = None
     variables: list[str] = field(default_factory=list)
+    sites: list[dict] = field(default_factory=list)     # per emit site: {"action": index into actions, -1 = trap only}
+    init: dict = field(default_factory=dict)            # the initial predicate: name, module and source span
+
 
     def meta(self) -> dict:
         return {
@@ -50,7 +54,7 @@ class LoweredModel:
             "actions": self.actions, "invariants": self.invariants, "constraints": self.constraints,
             "check_deadlock": self.check_deadlock, "max_fanout": self.max_fanout,
             "layout": self.layout, "digest": self.digest, "warnings": self.warnings,
-            "lowering_version": LOWERING_VERSION,
+            "lowering_version": LOWERING_VERSION, "sites": self.sites, "init": self.init,
         }
 
     def decode_state(self, words) -> dict:
@@ -466,6 +470,29 @@ def _init_states(lw: Lowerer, init_expr) -> list[dict]:
     return out
 
 
+_EMIT_LABEL = re.compile(r"sink\.emit\(n, (\d+)\);")
+
+
+def _site_action(body: list[str]) -> int:
+    """The action of an emit site: the label of the one sink.emit in its core (-1 for a core that only reports a
+    layout trap; reaching it fails the run)."""
+    labels = {int(x) for line in body for x in _EMIT_LABEL.findall(line)}
+    if len(labels) > 1:
+        raise LowerError("internal: an emit site carries more than one action label")
+    return labels.pop() if labels else -1
+
+
+def _init_info(lw: Lowerer, init_e, module: str) -> dict:
+    """Name and source span of the initial predicate (the <Init ...> line of a coverage report)."""
+    if init_e[0] == "id":
+        r = lw.root.resolve(init_e[1], None)
+        if r is not None and r.kind == "def":
+            d = r.defn
+            return {"name": d.name, "module": d.module or module, "line": d.line, "col": d.col,
+                    "end_line": d.end_line, "end_col": d.end_col}
+    return {"name": "Init", "module": module}
+
+
 def _resolve_init_next(lw: Lowerer):
     cfg, root = lw.cfg, lw.root
     if cfg.init and cfg.next:
@@ -742,6 +769,10 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     parts.append("#endif  // KMC_NO_ONE_PHASE")
     n_sites = len(site_bodies)
     parts.append(f"static constexpr int NUM_SITES = {n_sites};")
+    site_action = [_site_action(body) for body in site_bodies]
+    parts.append("/* action of every emit site (index into the model's actions; -1: the site only reports a layout trap) */")
+    parts.append("static constexpr int SITE_ACTION[NUM_SITES > 0 ? NUM_SITES : 1] = {" +
+                 (", ".join(str(a) for a in site_action) if site_action else "-1") + "};")
     parts.append(f"static constexpr int NUM_SITE_GROUPS = {len(site_groups)};")
     parts.append("static constexpr int SITE_GROUP_BEGIN[NUM_SITE_GROUPS + 1] = {" +
                  ", ".join(str(g["begin"]) for g in site_groups) + f", {n_sites}" + "};")
@@ -813,4 +844,5 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
         state_bits=lay.bits, init_states=init_words, actions=lw.actions or [{"name": "Next", "module": module}],
         invariants=list(cfg.invariants), constraints=list(cfg.constraints),
         check_deadlock=cfg.check_deadlock, max_fanout=max(1, max_fanout), warnings=lw.warnings,
-        digest=body_digest, lowerer=lw, variables=list(lw.variables))
+        digest=body_digest, lowerer=lw, variables=list(lw.variables),
+        sites=[{"action": a} for a in site_action], init=_init_info(lw, init_e, module))

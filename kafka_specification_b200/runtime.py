@@ -86,6 +86,8 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.kmc_stats.argtypes = [vp, ctypes.POINTER(Stats)]
     lib.kmc_level_widths.argtypes = [vp, u64p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
     lib.kmc_action_counts.argtypes = [vp, u64p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
+    lib.kmc_coverage.argtypes = [vp, u64p, u64p, ctypes.c_size_t, u64p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t),
+                                 ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_int32)]
     lib.kmc_violation.argtypes = [vp, ctypes.POINTER(Violation)]
     lib.kmc_trace_state.argtypes = [vp, ctypes.c_uint32, u64p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint32)]
     lib.kmc_copy_states.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp]
@@ -114,7 +116,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.kmc_shard_level_sync.argtypes = [vp, u64p]
     lib.kmc_shard_inbox_ptr.argtypes = [vp, ctypes.POINTER(vp)]
     lib.kmc_shard_open_peers_direct.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.c_uint32]
-    for fn in ("kmc_create", "kmc_model_info", "kmc_run", "kmc_stats", "kmc_level_widths", "kmc_action_counts",
+    for fn in ("kmc_create", "kmc_model_info", "kmc_run", "kmc_stats", "kmc_level_widths", "kmc_action_counts", "kmc_coverage",
                "kmc_violation", "kmc_trace_state", "kmc_copy_states", "kmc_copy_parents", "kmc_violation_record", "kmc_fpset_put", "kmc_fpset_contains",
                "kmc_fpset_size", "kmc_shard_begin", "kmc_shard_buffers", "kmc_shard_seed_init", "kmc_shard_expand",
                "kmc_shard_counts", "kmc_shard_reset_cand", "kmc_shard_insert", "kmc_shard_level_done", "kmc_shard_sync",
@@ -422,10 +424,39 @@ class Checker:
         return [int(buf[i]) for i in range(min(n.value, 4096))]
 
     def action_counts(self) -> dict:
-        buf = (ctypes.c_uint64 * 64)()
+        """Successors generated per action by the last run."""
+        cap = len(self.meta["actions"])
+        buf = (ctypes.c_uint64 * cap)()
         n = ctypes.c_size_t()
-        self._check(self.lib.kmc_action_counts(self.ctx, buf, 64, ctypes.byref(n)))
+        self._check(self.lib.kmc_action_counts(self.ctx, buf, cap, ctypes.byref(n)))
         return {a["name"]: int(buf[i]) for i, a in enumerate(self.meta["actions"]) if i < n.value}
+
+    def coverage(self) -> dict:
+        """TLC's coverage report of the last run:
+
+        * ``init``: the initial predicate (name, module, source span) with ``distinct`` / ``generated`` initial states;
+        * ``actions``: per action of model.json, ``{name, module, location, generated, distinct}``;
+        * ``sites``: successors generated per emit site of the lowered Next (model.json ``sites`` gives each one's action);
+        * ``complete``: False after recovering from a checkpoint without per-site counts (generated is then partial).
+
+        Generated per action is deterministic, and so is generated per site without SYMMETRY; distinct per action
+        depends on which generator of a new state won the insert (as in TLC with several workers).
+        """
+        acts, n_sites_meta = self.meta["actions"], len(self.meta.get("sites", []))
+        na, ns = len(acts), max(n_sites_meta, 1)
+        gen, dist, site = (ctypes.c_uint64 * na)(), (ctypes.c_uint64 * na)(), (ctypes.c_uint64 * ns)()
+        n_a, n_s, complete = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_int32()
+        self._check(self.lib.kmc_coverage(self.ctx, gen, dist, na, site, ns, ctypes.byref(n_a), ctypes.byref(n_s),
+                                          ctypes.byref(complete)))
+        if n_a.value != na or n_s.value != n_sites_meta:
+            raise KmcError(-7, "model.json does not describe the loaded model library's actions and emit sites")
+        st = self.stats()
+        actions = [{"name": a["name"], "module": a.get("module"), "location": {k: a[k] for k in ("line", "col", "end_line", "end_col") if k in a},
+                    "generated": int(gen[i]), "distinct": int(dist[i])} for i, a in enumerate(acts)]
+        init_distinct = st["distinct"] - sum(a["distinct"] for a in actions)
+        return {"init": {**self.meta.get("init", {"name": "Init"}), "distinct": init_distinct,
+                         "generated": len(self.meta["init_states"])},
+                "actions": actions, "sites": [int(site[i]) for i in range(n_s.value)], "complete": bool(complete.value)}
 
     def violation(self) -> dict | None:
         v = Violation()

@@ -2,7 +2,7 @@
 
     python -m kafka_specification_b200.tlc2 [-config F.cfg] [-workers N|auto] [-deadlock] [-continue]
                                              [-fpbits N] [-maxstates N] [-I dir] [-metadir d] [-checkpoint MIN]
-                                             [-recover DIR] [-spill] [-tool] SPEC
+                                             [-recover DIR] [-spill] [-coverage N] [-tool] SPEC
 
 ``SPEC`` is a module name or a path to ``SPEC.tla``; modules it EXTENDS / INSTANCEs are resolved
 from the same directory (and ``-I`` directories), like TLC does.  The spec and its ``.cfg`` are
@@ -11,6 +11,8 @@ the GPU through ``libkspecmc.so``, and the summary / error trace are printed in 
 ``-workers N`` selects N GPUs of this machine (fingerprint-sharded inside the library, option ``"gpus": N`` of
 kmc_create); ``-workers auto`` = one GPU (the GPU grid replaces TLC's worker threads).  ``-tool`` wraps the
 messages in TLC's tool-mode markers (``@!@!@STARTMSG code:class @!@!@`` ... ``@!@!@ENDMSG code @!@!@``).
+``-coverage N`` prints TLC's action-level coverage table ("distinct:generated" per action) once, at the end of the
+run (also after a violation): TLC repeats it every N minutes, but a search here takes seconds.
 
 Exit status follows TLC: 0 no error, 12 safety (invariant) violation, 11 deadlock,
 10 assumption failure, 150 spec/config error, 1 runtime failure (no GPU, table full, ...).
@@ -55,7 +57,7 @@ def parse_args(argv):
     ap.add_argument("-nowarning", action="store_true")
     ap.add_argument("-fp", type=int, default=0)
     ap.add_argument("-fpmem", type=float, default=0)
-    ap.add_argument("-coverage", type=int, default=0)
+    ap.add_argument("-coverage", type=int, default=0, help="print the coverage table at the end of the run (N > 0)")
     ap.add_argument("spec")
     return ap.parse_args(argv)
 
@@ -66,7 +68,10 @@ def parse_args(argv):
 EC = {"version": 2262, "mode": 2187, "sany_start": 2220, "sany_end": 2219, "starting": 2185, "init": 2189,
       "init_done": 2190, "inv_initial": 2107, "inv_behavior": 2110, "deadlock": 2114, "behavior": 2121,
       "state": 2217, "success": 2193, "collision": 2201, "stats": 2199, "depth": 2194, "finished": 2186,
-      "general": 1000}
+      "general": 1000,
+      # coverage (TLC >= 1.7, action level).  TLC publishes 2201 for the start of the coverage report; the entry
+      # "collision" above already uses 2201, and both are kept as they are.
+      "coverage_start": 2201, "coverage_init": 2772, "coverage_next": 2773, "coverage_end": 2202}
 _TOOL = False
 
 
@@ -90,6 +95,27 @@ def action_location(a: dict | None) -> str:
         return (f"<{a['name']} line {a['line']}, col {a['col']} to line {a['end_line']}, col {a['end_col']} "
                 f"of module {a['module']}>")
     return f"<{a['name']} of module {a.get('module', '?')}>"
+
+
+def coverage_lines(cov: dict, when: str) -> list[tuple[str, str]]:
+    """(EC kind, text) of TLC's coverage report for a ``Checker.coverage()`` dict: the initial predicate, then one
+    line per action in model.json order (actions that never fired included, as 0:0)."""
+    def loc(a):
+        return action_location({"name": a["name"], "module": a.get("module") or "?", **a.get("location", {})})
+    init = cov["init"]
+    out = [("coverage_start", f"The coverage statistics at {when}"),
+           ("coverage_init", f"{action_location(init)}: {init['distinct']}:{init['generated']}")]
+    out += [("coverage_next", f"{loc(a)}: {a['distinct']}:{a['generated']}") for a in cov["actions"]]
+    out.append(("coverage_end", "End of statistics."))
+    return out
+
+
+def print_coverage(cov: dict):
+    if not cov["complete"]:
+        msg("general", "Warning: the run recovered from a checkpoint without per-site counts; the generated counts "
+                       "below cover only the levels searched since.")
+    for kind, text in coverage_lines(cov, time.strftime("%Y-%m-%d %H:%M:%S")):
+        msg(kind, text)
 
 
 def main(argv=None) -> int:
@@ -197,6 +223,8 @@ def main(argv=None) -> int:
         else:
             p128 = collision_probability(r.distinct, r.generated) / 2.0 ** 65
             msg("collision", f"  calculated (optimistic):  val = {p128:.1E} (128-bit fingerprints)")
+    if a.coverage > 0:
+        print_coverage(ck.coverage())
     msg("stats", f"{r.generated} states generated, {r.distinct} distinct states found, {r.queue} states left on queue.")
     if r.complete:
         msg("depth", f"The depth of the complete state graph search is {r.depth}.")
