@@ -1128,8 +1128,9 @@ struct Engine {
   std::vector<uint64_t> viol_words;     // the offending state itself and its parent/action word
   uint64_t viol_meta = 0;
   bool ran = false;
-  uint64_t level_first = 0, level_count = 0;   // shard API
-  uint64_t shard_levels = 0;
+  // the level cursor: the states [level_first, level_first + level_count) form BFS level `level`, the one expanded
+  // next (level 0: nothing inserted yet)
+  uint64_t level_first = 0, level_count = 0, level = 0;
   std::string last_error;
 
   Params params() const {
@@ -1343,8 +1344,7 @@ static int engine_reset(Engine& E) {
   E.trace_actions.clear();
   memset(&E.viol, 0, sizeof(E.viol));
   E.viol.invariant = -1;
-  E.level_first = E.level_count = 0;
-  E.shard_levels = 0;
+  E.level_first = E.level_count = E.level = 0;
   E.store_base = 0;
   E.host_store.clear();
   E.host_parent.clear();
@@ -1357,9 +1357,18 @@ static int engine_reset(Engine& E) {
   return KMC_OK;
 }
 
-// host copy of the coverage counters (the caller has just read them from the device)
-static void keep_coverage(Engine& E, const DevCounters& h) {
-  std::lock_guard<std::mutex> g(E.mu);
+// The stats and coverage that come from the device counters (the caller holds E.mu).  kmc_run clamps distinct to
+// the store (`clamp`): without spill, a run that overflowed the store counted states it could not keep.
+static void publish(Engine& E, const DevCounters& h, bool clamp) {
+  kmc_stats_t& st = E.stats;
+  st.distinct = clamp && !E.spill ? std::min<uint64_t>(h.store_tail, E.max_states) : h.store_tail;
+  st.generated = h.generated;
+  st.deadlocks = h.deadlocks;
+  st.out_of_model = h.out_of_model;
+  st.probes = h.probes;
+  st.table_slots = E.table_slots;
+  st.slot_bytes = SLOT_BYTES;
+  st.max_states = E.max_states;
   E.site_generated.assign(h.site_generated, h.site_generated + M::NUM_SITES);
   E.action_distinct.assign(h.action_distinct, h.action_distinct + M::NUM_ACTIONS);
 }
@@ -1451,29 +1460,40 @@ static int reset_cand(Engine& E) {
   return KMC_OK;
 }
 
-// State / parent word by GLOBAL index: from the host spill below store_base, else from the device ring.
-static int fetch_state(Engine& E, uint64_t idx, uint64_t* words, uint64_t* meta) {
-  if (idx < E.store_base) {
-    memcpy(words, E.host_store.data() + idx * W, W * 8);
-    *meta = E.host_parent[idx];
-    return KMC_OK;
+// The store by GLOBAL index: below store_base it is the host spill, from there on the device store, a ring when
+// spilling.  Returns the device slot of index g and how many indices from g on, up to `end`, precede the ring's wrap.
+static uint64_t ring_run(const Engine& E, uint64_t g, uint64_t end, uint64_t* slot) {
+  *slot = E.spill ? (g & (E.max_states - 1)) : g;
+  return E.spill ? std::min<uint64_t>(end - g, E.max_states - *slot) : end - g;
+}
+
+// Store range [first, first + count) -> host buffers; either may be null.  The device part is copied synchronously,
+// after the stream synchronisation of the counter read that made the range known.
+static int read_range(Engine& E, uint64_t first, uint64_t count, uint64_t* states, uint64_t* parents) {
+  const uint64_t end = first + count, host_end = std::min(end, std::max(first, E.store_base));
+  if (host_end > first) {
+    if (states) memcpy(states, E.host_store.data() + first * W, (host_end - first) * W * 8);
+    if (parents) memcpy(parents, E.host_parent.data() + first, (host_end - first) * 8);
   }
-  const uint64_t slot = E.spill ? (idx & (E.max_states - 1)) : idx;
-  CK(cudaMemcpy(words, E.store + slot * W, W * 8, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(meta, E.parent + slot, 8, cudaMemcpyDeviceToHost));
+  for (uint64_t g = host_end, slot, n; g < end; g += n) {
+    n = ring_run(E, g, end, &slot);
+    if (states) CK(cudaMemcpy(states + (g - first) * W, E.store + slot * W, n * W * 8, cudaMemcpyDeviceToHost));
+    if (parents) CK(cudaMemcpy(parents + (g - first), E.parent + slot, n * 8, cudaMemcpyDeviceToHost));
+  }
   return KMC_OK;
 }
 
-// device ring range [first, first + count) (global indices, all on the device) -> host buffers
-static int copy_ring_range(Engine& E, uint64_t first, uint64_t count, uint64_t* states, uint64_t* parents) {
-  uint64_t done = 0;
-  while (done < count) {
-    const uint64_t g = first + done;
-    const uint64_t slot = E.spill ? (g & (E.max_states - 1)) : g;
-    const uint64_t n = E.spill ? std::min<uint64_t>(count - done, E.max_states - slot) : count - done;
-    if (states) CK(cudaMemcpy(states + done * W, E.store + slot * W, n * W * 8, cudaMemcpyDeviceToHost));
-    if (parents) CK(cudaMemcpy(parents + done, E.parent + slot, n * 8, cudaMemcpyDeviceToHost));
-    done += n;
+// host buffers -> store range [first, first + count) (recover); the device part is copied on the engine stream
+static int write_range(Engine& E, uint64_t first, uint64_t count, const uint64_t* states, const uint64_t* parents) {
+  const uint64_t end = first + count, host_end = std::min(end, std::max(first, E.store_base));
+  if (host_end > first) {
+    memcpy(E.host_store.data() + first * W, states, (host_end - first) * W * 8);
+    memcpy(E.host_parent.data() + first, parents, (host_end - first) * 8);
+  }
+  for (uint64_t g = host_end, slot, n; g < end; g += n) {
+    n = ring_run(E, g, end, &slot);
+    CK(cudaMemcpyAsync(E.store + slot * W, states + (g - first) * W, n * W * 8, cudaMemcpyHostToDevice, E.stream));
+    CK(cudaMemcpyAsync(E.parent + slot, parents + (g - first), n * 8, cudaMemcpyHostToDevice, E.stream));
   }
   return KMC_OK;
 }
@@ -1481,10 +1501,10 @@ static int copy_ring_range(Engine& E, uint64_t first, uint64_t count, uint64_t* 
 // Spill: everything below the level that is expanded next moves to host memory and its ring slots become free.
 static int spill_below(Engine& E, uint64_t level_first) {
   if (!E.spill || level_first <= E.store_base) return KMC_OK;
-  const uint64_t n = level_first - E.store_base;
+  const uint64_t base = E.store_base;
   E.host_store.resize(level_first * W);
   E.host_parent.resize(level_first);
-  int rc = copy_ring_range(E, E.store_base, n, E.host_store.data() + E.store_base * W, E.host_parent.data() + E.store_base);
+  int rc = read_range(E, base, level_first - base, E.host_store.data() + base * W, E.host_parent.data() + base);
   if (rc) return rc;
   E.store_base = level_first;
   return KMC_OK;
@@ -1493,10 +1513,7 @@ static int spill_below(Engine& E, uint64_t level_first) {
 // ---- checkpoint / recover (TLC -checkpoint / -recover): written at a level boundary -------------------------------
 // <dir>/checkpoint.meta  text: key value per line;  <dir>/checkpoint.bin  states [0, tail) then parent words [0, tail).
 // The fingerprint set is not stored: it is rebuilt from the states on recover (and may then have another size).
-struct LevelCursor {
-  uint64_t level_first, level_end, level;
-};
-static int write_checkpoint(Engine& E, const DevCounters& h, const LevelCursor& lc) {
+static int write_checkpoint(Engine& E, const DevCounters& h) {
   const std::string meta = E.checkpoint_dir + "/checkpoint.meta", bin = E.checkpoint_dir + "/checkpoint.bin";
   const std::string tmp = bin + ".tmp";
   FILE* f = fopen(tmp.c_str(), "wb");
@@ -1504,14 +1521,18 @@ static int write_checkpoint(Engine& E, const DevCounters& h, const LevelCursor& 
     E.last_error = "cannot write " + tmp;
     return KMC_E_BADARG;
   }
-  const uint64_t tail = h.store_tail;
-  std::vector<uint64_t> st((size_t)(tail - E.store_base) * W), pa((size_t)(tail - E.store_base));
-  int rc = copy_ring_range(E, E.store_base, tail - E.store_base, st.data(), pa.data());
-  if (rc) { fclose(f); return rc; }
-  bool ok = fwrite(E.host_store.data(), 8, (size_t)E.store_base * W, f) == (size_t)E.store_base * W &&
-            fwrite(st.data(), 8, st.size(), f) == st.size() &&
-            fwrite(E.host_parent.data(), 8, (size_t)E.store_base, f) == (size_t)E.store_base &&
-            fwrite(pa.data(), 8, pa.size(), f) == pa.size();
+  // the states, then the parent words, through a bounded buffer: with spill most of the store is in host memory
+  const uint64_t tail = h.store_tail, piece = 1 << 20;
+  std::vector<uint64_t> buf;
+  bool ok = true;
+  for (int parents = 0; parents < 2 && ok; ++parents)
+    for (uint64_t g = 0; g < tail && ok; g += piece) {
+      const uint64_t n = std::min(piece, tail - g);
+      buf.resize(parents ? n : n * W);
+      int rc = read_range(E, g, n, parents ? nullptr : buf.data(), parents ? buf.data() : nullptr);
+      if (rc) { fclose(f); return rc; }
+      ok = fwrite(buf.data(), 8, buf.size(), f) == buf.size();
+    }
   ok = (fclose(f) == 0) && ok;
   if (!ok || rename(tmp.c_str(), bin.c_str()) != 0) {
     E.last_error = "short write on " + tmp;
@@ -1521,8 +1542,8 @@ static int write_checkpoint(Engine& E, const DevCounters& h, const LevelCursor& 
   if (!f) return KMC_E_BADARG;
   fprintf(f, "model %s\ndigest %s\nwords %d\ntail %llu\nlevel_first %llu\nlevel_end %llu\nlevel %llu\ngenerated %llu\n"
              "deadlocks %llu\nout_of_model %llu\nprobes %llu\nsite_generated",
-          KMC_MODEL_NAME, KMC_MODEL_DIGEST, W, (unsigned long long)tail, (unsigned long long)lc.level_first,
-          (unsigned long long)lc.level_end, (unsigned long long)lc.level, (unsigned long long)h.generated,
+          KMC_MODEL_NAME, KMC_MODEL_DIGEST, W, (unsigned long long)tail, (unsigned long long)E.level_first,
+          (unsigned long long)(E.level_first + E.level_count), (unsigned long long)E.level, (unsigned long long)h.generated,
           (unsigned long long)h.deadlocks, (unsigned long long)h.out_of_model, (unsigned long long)h.probes);
   // (before widths: a reader stops at widths.  Distinct per action is not written: it is the histogram of the
   // parent words, which recover reads anyway)
@@ -1536,7 +1557,8 @@ static int write_checkpoint(Engine& E, const DevCounters& h, const LevelCursor& 
   return KMC_OK;
 }
 
-static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
+// Sets the level cursor to the level the checkpoint expands next, and *h to the counters it restored.
+static int read_checkpoint(Engine& E, DevCounters* h) {
   const std::string meta = E.recover_dir + "/checkpoint.meta", bin = E.recover_dir + "/checkpoint.bin";
   FILE* f = fopen(meta.c_str(), "r");
   if (!f) {
@@ -1544,7 +1566,7 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
     return KMC_E_BADARG;
   }
   char key[64], val[256];
-  unsigned long long tail = 0, words = 0;
+  unsigned long long tail = 0, words = 0, level_first = 0, level_end = 0, level = 1;
   std::string digest;
   bool have_sites = false;
   memset(h, 0, sizeof(*h));
@@ -1566,9 +1588,9 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
     if (!strcmp(key, "digest")) digest = val;
     else if (!strcmp(key, "words")) words = v;
     else if (!strcmp(key, "tail")) tail = v;
-    else if (!strcmp(key, "level_first")) lc->level_first = v;
-    else if (!strcmp(key, "level_end")) lc->level_end = v;
-    else if (!strcmp(key, "level")) lc->level = v;
+    else if (!strcmp(key, "level_first")) level_first = v;
+    else if (!strcmp(key, "level_end")) level_end = v;
+    else if (!strcmp(key, "level")) level = v;
     else if (!strcmp(key, "generated")) h->generated = v;
     else if (!strcmp(key, "deadlocks")) h->deadlocks = v;
     else if (!strcmp(key, "out_of_model")) h->out_of_model = v;
@@ -1581,7 +1603,7 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
   }
   h->store_tail = tail;
   // states below the level to expand go to the host (spill) or, without spill, everything to the device
-  const uint64_t keep_from = E.spill ? lc->level_first : 0;
+  const uint64_t keep_from = E.spill ? level_first : 0;
   if (tail - keep_from > E.max_states) {
     E.last_error = "checkpoint does not fit the state store (raise max_states or use spill)";
     return KMC_E_STORE_FULL;
@@ -1607,16 +1629,12 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
   if (!have_sites) memset(h->site_generated, 0, sizeof(h->site_generated));
   E.coverage_complete = have_sites;      // a checkpoint written before the per-site counts existed: generated is partial
   E.store_base = keep_from;
-  E.host_store.assign(st.begin(), st.begin() + (size_t)keep_from * W);
-  E.host_parent.assign(pa.begin(), pa.begin() + (size_t)keep_from);
-  // device window
-  for (uint64_t g = keep_from; g < tail;) {
-    const uint64_t slot = E.spill ? (g & (E.max_states - 1)) : g;
-    const uint64_t n = E.spill ? std::min<uint64_t>(tail - g, E.max_states - slot) : tail - g;
-    CK(cudaMemcpyAsync(E.store + slot * W, st.data() + g * W, n * W * 8, cudaMemcpyHostToDevice, E.stream));
-    CK(cudaMemcpyAsync(E.parent + slot, pa.data() + g, n * 8, cudaMemcpyHostToDevice, E.stream));
-    g += n;
-  }
+  E.host_store.resize((size_t)keep_from * W);
+  E.host_parent.resize((size_t)keep_from);
+  int rc = write_range(E, 0, tail, st.data(), pa.data());
+  if (rc) return rc;
+  // the counters in one copy, before the rebuild: k_rebuild sets `fail` when the set overflows
+  CK(cudaMemcpyAsync(E.ctr, h, sizeof(*h), cudaMemcpyHostToDevice, E.stream));
   // rebuild the set: every stored state is inserted once, in batches through the candidate buffer
   Params p = E.params();
   const uint64_t batch = E.region_rows * ROW / W;
@@ -1626,18 +1644,13 @@ static int read_checkpoint(Engine& E, DevCounters* h, LevelCursor* lc) {
     k_rebuild<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(p, E.cand, n);
     CK(cudaStreamSynchronize(E.stream));
   }
-  CK(cudaMemcpyAsync(&E.ctr->store_tail, &h->store_tail, 8, cudaMemcpyHostToDevice, E.stream));
-  CK(cudaMemcpyAsync(&E.ctr->generated, &h->generated, 8, cudaMemcpyHostToDevice, E.stream));
-  CK(cudaMemcpyAsync(&E.ctr->deadlocks, &h->deadlocks, 8, cudaMemcpyHostToDevice, E.stream));
-  CK(cudaMemcpyAsync(&E.ctr->out_of_model, &h->out_of_model, 8, cudaMemcpyHostToDevice, E.stream));
-  CK(cudaMemcpyAsync(&E.ctr->probes, &h->probes, 8, cudaMemcpyHostToDevice, E.stream));
-  CK(cudaMemcpyAsync(E.ctr->site_generated, h->site_generated, sizeof(h->site_generated), cudaMemcpyHostToDevice, E.stream));
-  CK(cudaMemcpyAsync(E.ctr->action_distinct, h->action_distinct, sizeof(h->action_distinct), cudaMemcpyHostToDevice, E.stream));
-  CK(cudaStreamSynchronize(E.stream));
   DevCounters now;
-  int rc = read_counters(E, &now);
-  if (rc) return rc;
-  return fail_to_error(now.fail);
+  if ((rc = read_counters(E, &now))) return rc;
+  if ((rc = fail_to_error(now.fail))) return rc;
+  E.level_first = level_first;
+  E.level_count = level_end - level_first;
+  E.level = level;
+  return KMC_OK;
 }
 
 // Picks the violator with the smallest fingerprint (deadlocks, which belong to the level being
@@ -1669,10 +1682,7 @@ static int build_trace(Engine& E, const DevCounters& h, uint64_t level) {
     uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
     if (prank != E.rank || idx - E.store_base >= E.max_states && idx >= E.store_base) break;  // parent lives on another rank
     std::vector<uint64_t> st(W);
-    {
-      int frc = fetch_state(E, idx, st.data(), &meta);
-      if (frc) return frc;
-    }
+    if (int rc = read_range(E, idx, 1, st.data(), &meta)) return rc;
     rev.push_back(st);
     rev_act.push_back((uint32_t)(meta >> 56));
   }
@@ -1699,6 +1709,29 @@ static void accumulate_timing(Engine& E, kmc_stats_t& st) {
   }
 }
 
+// End of a level: invariants on the states it added (`inv_bound` bounds their grid), one counter read, the cursor
+// moves on to those states, stats and coverage are published, and the first violation builds the trace.
+// kmc_run (`shard` false) reports distinct clamped to the store and the queue, lists the widths of the levels it
+// expands itself and does not trace a failed level; the shard calls list every non-empty level they find.
+static int end_level(Engine& E, uint64_t inv_bound, bool shard, DevCounters& h) {
+  const uint64_t end = E.level_first + E.level_count;
+  int rc = launch_invariants(E, end, inv_bound);
+  if (rc || (rc = read_counters(E, &h))) return rc;
+  const uint64_t level = E.level++;
+  E.level_first = end;
+  E.level_count = h.store_tail - end;
+  {
+    std::lock_guard<std::mutex> g(E.mu);
+    publish(E, h, !shard);
+    if (shard && E.level_count) E.widths.push_back(E.level_count);
+    E.stats.depth = E.widths.size();
+    if (shard) E.stats.levels = E.stats.depth;
+    else E.stats.queue = E.level_count;
+  }
+  if (h.viol_count && E.viol.kind == KMC_RESULT_OK && (shard || !h.fail)) build_trace(E, h, level);
+  return KMC_OK;
+}
+
 static int engine_run(Engine& E) {
   auto t0 = std::chrono::steady_clock::now();
   int rc = engine_reset(E);
@@ -1709,73 +1742,43 @@ static int engine_run(Engine& E) {
   }
   CK(cudaEventRecord(E.ev_begin, E.stream));
   DevCounters h;
-  uint64_t level_first = 0, level_end = 0, level = 1;
   bool stopped = false;
   int err = 0;
   E.last_checkpoint = std::chrono::steady_clock::now();
   if (!E.recover_dir.empty()) {
     // -recover: continue from the level boundary a checkpoint was written at
-    LevelCursor lc{0, 0, 1};
-    if ((rc = read_checkpoint(E, &h, &lc))) return rc;
-    level_first = lc.level_first;
-    level_end = lc.level_end;
-    level = lc.level;
+    if ((rc = read_checkpoint(E, &h))) return rc;
   } else {
-    rc = seed_init(E);
-    if (rc) return rc;
-    rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, M::NUM_INIT);
-    if (rc) return rc;
-    if ((rc = launch_invariants(E, 0, M::NUM_INIT))) return rc;
-    rc = read_counters(E, &h);
-    if (rc) return rc;
-    level_end = h.store_tail;
+    if ((rc = seed_init(E))) return rc;
+    if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, M::NUM_INIT))) return rc;
+    if ((rc = end_level(E, M::NUM_INIT, false, h))) return rc;
     err = fail_to_error(h.fail);
-    if (!err && h.viol_count) {
-      build_trace(E, h, 0);
-      if (!E.cont) stopped = true;
-    }
+    if (!err && h.viol_count && !E.cont) stopped = true;
   }
-  while (!err && !stopped && level_end > level_first) {
-    E.widths.push_back(level_end - level_first);
-    if ((rc = spill_below(E, level_first))) return rc;         // (no-op unless spilling)
-    for (uint64_t off = level_first, cnt; off < level_end; off += cnt) {
-      cnt = std::min<uint64_t>(E.chunk_states, level_end - off);
-      // a chunk never crosses the wrap of the ring store
-      if (E.spill) cnt = std::min<uint64_t>(cnt, E.max_states - (off & (E.max_states - 1)));
+  while (!err && !stopped && E.level_count) {
+    E.widths.push_back(E.level_count);
+    if ((rc = spill_below(E, E.level_first))) return rc;         // (no-op unless spilling)
+    const uint64_t level_end = E.level_first + E.level_count;
+    for (uint64_t off = E.level_first, slot, cnt; off < level_end; off += cnt) {
+      cnt = std::min<uint64_t>(E.chunk_states, ring_run(E, off, level_end, &slot));   // a chunk never crosses the wrap
       if ((rc = reset_cand(E))) return rc;
       if ((rc = launch_expand(E, off, cnt))) return rc;
       if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, cnt * (uint64_t)E.fanout_bound))) return rc;
     }
-    if ((rc = launch_invariants(E, level_end, (level_end - level_first) * 2))) return rc;
-    if ((rc = read_counters(E, &h))) return rc;
+    if ((rc = end_level(E, E.level_count * 2, false, h))) return rc;
     err = fail_to_error(h.fail);
-    {
-      std::lock_guard<std::mutex> g(E.mu);
-      E.stats.distinct = E.spill ? h.store_tail : std::min<uint64_t>(h.store_tail, E.max_states);
-      E.stats.generated = h.generated;
-      E.stats.depth = level;
-      E.stats.queue = h.store_tail - level_end;
+    if (!err && h.viol_count && !E.cont) {
+      stopped = true;
+      break;
     }
-    if (!err && h.viol_count && E.viol.kind == KMC_RESULT_OK) {
-      build_trace(E, h, level);
-      if (!E.cont) {
-        stopped = true;
-        level_first = level_end;
-        level_end = h.store_tail;
-        break;
-      }
-    }
-    level_first = level_end;
-    level_end = h.store_tail;
-    ++level;
-    if (!err && !E.checkpoint_dir.empty() && level_end > level_first) {
+    if (!err && !E.checkpoint_dir.empty() && E.level_count) {
       const double mins = std::chrono::duration<double>(std::chrono::steady_clock::now() - E.last_checkpoint).count() / 60.0;
       if (mins >= E.checkpoint_minutes) {
-        if ((rc = spill_below(E, level_first))) return rc;
-        if ((rc = write_checkpoint(E, h, LevelCursor{level_first, level_end, level}))) return rc;
+        if ((rc = spill_below(E, E.level_first))) return rc;
+        if ((rc = write_checkpoint(E, h))) return rc;
       }
     }
-    if (E.stop_after_states && h.store_tail >= E.stop_after_states && level_end > level_first) {
+    if (E.stop_after_states && h.store_tail >= E.stop_after_states && E.level_count) {
       stopped = true;          // bounded throughput run: the queue is reported, no error
       break;
     }
@@ -1787,25 +1790,16 @@ static int engine_run(Engine& E) {
   auto t1 = std::chrono::steady_clock::now();
   {
     std::lock_guard<std::mutex> g(E.mu);
+    publish(E, h, true);
     kmc_stats_t& st = E.stats;
-    st.distinct = E.spill ? h.store_tail : std::min<uint64_t>(h.store_tail, E.max_states);
-    st.generated = h.generated;
-    st.queue = stopped ? (level_end - level_first) : 0;
-    st.depth = E.widths.size();
-    st.deadlocks = h.deadlocks;
-    st.out_of_model = h.out_of_model;
-    st.probes = h.probes;
-    st.levels = E.widths.size();
+    st.queue = stopped ? E.level_count : 0;
+    st.depth = st.levels = E.widths.size();
     st.gpu_ms_total = total_ms;
     st.wall_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
-    st.table_slots = E.table_slots;
-    st.slot_bytes = SLOT_BYTES;
-    st.max_states = E.max_states;
     st.complete = (!err && !stopped) ? 1 : 0;
     if (E.timing) accumulate_timing(E, st);
     E.ran = true;
   }
-  keep_coverage(E, h);
   return err;
 }
 
@@ -1958,7 +1952,7 @@ int kmcm_coverage(const kmcm_ctx* c, uint64_t* action_gen, uint64_t* action_dist
 
 int kmcm_violation(const kmcm_ctx* c, kmc_violation_t* out) {
   if (!c || !out) return KMC_E_BADARG;
-  if (!E.ran && E.shard_levels == 0) return KMC_E_STATE;
+  if (!E.ran && E.level == 0) return KMC_E_STATE;
   *out = E.viol;
   return KMC_OK;
 }
@@ -1980,40 +1974,20 @@ int kmcm_violation_record(const kmcm_ctx* c, uint64_t* words, size_t cap_words, 
   return KMC_OK;
 }
 
-int kmcm_copy_parents(const kmcm_ctx* c_, uint64_t first, uint64_t count, uint64_t* buf) {
+// states and / or parent words [first, first + count) by global index
+static int copy_store(const kmcm_ctx* c_, uint64_t first, uint64_t count, uint64_t* states, uint64_t* parents) {
   kmcm_ctx* c = const_cast<kmcm_ctx*>(c_);
-  if (!c || !buf) return KMC_E_BADARG;
+  if (!c || !(states || parents)) return KMC_E_BADARG;
   if (!c->ranks.empty()) return KMC_E_STATE;      // per-rank stores: address a rank's own context
   CK(cudaSetDevice(E.device));
-  if (E.spill) {
-    std::vector<uint64_t> tmp(W);
-    for (uint64_t i = 0; i < count; ++i) {
-      int rc = fetch_state(E, first + i, tmp.data(), buf + i);
-      if (rc) return rc;
-    }
-    return KMC_OK;
-  }
-  if (first + count > E.max_states) return KMC_E_BADARG;
-  CK(cudaMemcpy(buf, E.parent + first, count * 8, cudaMemcpyDeviceToHost));
-  return KMC_OK;
+  if (!E.spill && first + count > E.max_states) return KMC_E_BADARG;
+  return read_range(E, first, count, states, parents);
 }
-
-int kmcm_copy_states(const kmcm_ctx* c_, uint64_t first, uint64_t count, uint64_t* buf) {
-  kmcm_ctx* c = const_cast<kmcm_ctx*>(c_);
-  if (!c || !buf) return KMC_E_BADARG;
-  if (!c->ranks.empty()) return KMC_E_STATE;
-  CK(cudaSetDevice(E.device));
-  if (E.spill) {
-    uint64_t meta;
-    for (uint64_t i = 0; i < count; ++i) {
-      int rc = fetch_state(E, first + i, buf + i * W, &meta);
-      if (rc) return rc;
-    }
-    return KMC_OK;
-  }
-  if (first + count > E.max_states) return KMC_E_BADARG;
-  CK(cudaMemcpy(buf, E.store + first * W, count * W * 8, cudaMemcpyDeviceToHost));
-  return KMC_OK;
+int kmcm_copy_parents(const kmcm_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) {
+  return copy_store(c, first, count, nullptr, buf);
+}
+int kmcm_copy_states(const kmcm_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) {
+  return copy_store(c, first, count, buf, nullptr);
 }
 
 const char* kmcm_strerror(const kmcm_ctx* c, int code) {
@@ -2071,7 +2045,6 @@ int kmcm_shard_begin(kmcm_ctx* c) {
   int rc = engine_reset(E);
   if (rc) return rc;
   E.inbox_buf = 0;
-  E.shard_levels = 0;
   E.ran = false;
   CK(cudaEventRecord(E.ev_begin, E.stream));
   return KMC_OK;
@@ -2136,31 +2109,10 @@ int kmcm_shard_insert(kmcm_ctx* c, const uint64_t* rows_dev, uint64_t rows, uint
 int kmcm_shard_level_done(kmcm_ctx* c, uint64_t* level_first, uint64_t* level_count) {
   if (!c) return KMC_E_BADARG;
   DevCounters h;
-  int rc = launch_invariants(E, E.level_first + E.level_count, std::max<uint64_t>(E.level_count * 2, 1024));
+  int rc = end_level(E, std::max<uint64_t>(E.level_count * 2, 1024), true, h);
   if (rc) return rc;
-  rc = read_counters(E, &h);
-  if (rc) return rc;
-  uint64_t prev_end = E.level_first + E.level_count;
-  E.level_first = prev_end;
-  E.level_count = h.store_tail - prev_end;
-  E.shard_levels++;
   if (level_first) *level_first = E.level_first;
   if (level_count) *level_count = E.level_count;
-  {
-    std::lock_guard<std::mutex> g(E.mu);
-    E.stats.distinct = h.store_tail;
-    E.stats.generated = h.generated;
-    E.stats.deadlocks = h.deadlocks;
-    E.stats.out_of_model = h.out_of_model;
-    E.stats.probes = h.probes;
-    E.stats.table_slots = E.table_slots;
-    E.stats.slot_bytes = SLOT_BYTES;
-    E.stats.max_states = E.max_states;
-    if (E.level_count) E.widths.push_back(E.level_count);
-    E.stats.levels = E.stats.depth = E.widths.size();
-  }
-  keep_coverage(E, h);
-  if (h.viol_count && E.viol.kind == KMC_RESULT_OK) build_trace(E, h, E.shard_levels - 1);
   return fail_to_error(h.fail);
 }
 
@@ -2312,7 +2264,7 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
   const uint64_t prev_end = E.level_first + E.level_count;
   E.level_first = prev_end;
   E.level_count = mine[1];
-  E.shard_levels++;
+  E.level++;
   {
     std::lock_guard<std::mutex> g(E.mu);
     E.stats.distinct = mine[3];
@@ -2327,7 +2279,7 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
   if (mine[2] && E.viol.kind == KMC_RESULT_OK) {
     DevCounters h;
     if ((rc = read_counters(E, &h))) return rc;
-    build_trace(E, h, E.shard_levels - 1);
+    build_trace(E, h, E.level - 1);
   }
   return fail_to_error(mine[5]);
 }
@@ -2361,20 +2313,13 @@ int kmcm_shard_open_peers_direct(kmcm_ctx* c, void* const* inboxes, const int* d
 int kmcm_shard_sync(kmcm_ctx* c) {
   if (!c) return KMC_E_BADARG;
   CK(cudaEventRecord(E.ev_end, E.stream));
-  DevCounters hc;
-  {
-    int rc = read_counters(E, &hc);              // synchronises the stream
-    if (rc) return rc;
-    keep_coverage(E, hc);
-    std::lock_guard<std::mutex> g(E.mu);
-    E.stats.probes = hc.probes;
-    E.stats.out_of_model = hc.out_of_model;
-    E.stats.generated = hc.generated;
-    E.stats.deadlocks = hc.deadlocks;
-  }
+  DevCounters h;
+  int rc = read_counters(E, &h);              // synchronises the stream
+  if (rc) return rc;
   float total_ms = 0;
   cudaEventElapsedTime(&total_ms, E.ev_begin, E.ev_end);
   std::lock_guard<std::mutex> g(E.mu);
+  publish(E, h, false);
   E.stats.gpu_ms_total = total_ms;
   if (E.timing) accumulate_timing(E, E.stats);
   return KMC_OK;
