@@ -156,7 +156,8 @@ int kmc_violation_record(const kmc_ctx* ctx, uint64_t* words, size_t cap_words, 
 const char* kmc_strerror(const kmc_ctx* ctx, int code);
 
 /* ---- fingerprint set alone (FPSet.put / contains / size) ------------------------------ */
-/* fps: n host fingerprints; out_seen[i] = 1 if already present (TLC's put() contract).     */
+/* fps: n host fingerprints; out_seen[i] = 1 if already present (TLC's put() contract).
+ * Fingerprint 0 is stored as 1 (0 marks an empty 8-byte slot), so 0 and 1 are the same key.  */
 int kmc_fpset_put(kmc_ctx* ctx, const uint64_t* fps, size_t n, uint8_t* out_seen);
 int kmc_fpset_contains(kmc_ctx* ctx, const uint64_t* fps, size_t n, uint8_t* out_present);
 int kmc_fpset_size(const kmc_ctx* ctx, uint64_t* out);

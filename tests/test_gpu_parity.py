@@ -17,7 +17,8 @@ pytestmark = pytest.mark.gpu
 
 ALL_MODELS = ["idsequence", "frl_tiny", "frl_3x4x2", "frl_3x4x3", "kip320_n2", "trunchw_n2", "kip101_n2", "kip279_n2",
               "firsttry_n2", "kip320_small", "trunchw_small", "kip101_small", "kip279_small", "firsttry_small",
-              "asyncisr_v2", "asyncisr_small", "kip320sym_n2", "kip320sym_small", "minilock", "kip320_with279_small"]
+              "asyncisr_v2", "asyncisr_small", "kip320sym_n2", "kip320sym_small", "minilock", "kip320_with279_small",
+              "asyncisr_w3"]
 DIGEST_MODELS = ["minilock", "idsequence", "frl_tiny", "kip320_n2", "trunchw_n2", "kip101_n2", "kip279_n2", "firsttry_n2",
                  "asyncisr_v2", "asyncisr_small", "kip320_small", "frl_3x4x2", "frl_3x4x3"]
 
@@ -210,8 +211,8 @@ def test_kip320_needs_its_epoch_check_as_the_reference_says(goldens):
 
 def test_exactness_of_the_set_by_state_width():
     """<= 63 bits: bijective 64-bit fingerprint; two words: the packed state itself is the 128-bit key (exact);
-    wider: 128-bit fingerprint."""
-    for name, exact, slot in (("frl_3x4x3", 1, 8), ("kip320_small", 1, 16), ("asyncisr_small", 1, 16)):
+    wider (asyncisr_w3: three words): 128-bit fingerprint."""
+    for name, exact, slot in (("frl_3x4x3", 1, 8), ("kip320_small", 1, 16), ("asyncisr_small", 1, 16), ("asyncisr_w3", 0, 16)):
         with checker(name, cont=True) as ck:
             r = ck.run()
             assert (ck.info.exact, r.stats["slot_bytes"]) == (exact, slot), name

@@ -18,7 +18,7 @@ DIRS = [REFERENCE, os.path.join(ROOT, "models")]
 SMALL = ["idsequence", "frl_tiny", "frl_3x4x2", "kip320_n2", "trunchw_n2", "kip101_n2", "kip279_n2", "firsttry_n2",
          "asyncisr_v2", "asyncisr_small", "kip320sym_n2"]
 MEDIUM = ["kip320_small", "trunchw_small", "kip101_small", "kip279_small", "firsttry_small", "kip320sym_small",
-          "kip320_with279_small"]
+          "kip320_with279_small", "asyncisr_w3"]
 if os.environ.get("KSPEC_SLOW_TESTS") == "1":
     MEDIUM.append("frl_3x4x3")       # 28 M successors on the sequential host harness: 2 more minutes (digest verified once, round 2)
 
