@@ -9,9 +9,10 @@
 //                   complete path conditions of its states (site_mask), then warps run the straight-line
 //                   bodies of the enabled (state, site) pairs one site at a time (site_body).  Successor
 //                   rows (state words + parent/action word) are staged per warp in shared memory and
-//                   flushed in bulk: into the local candidate buffer (one rank), into per-owner regions
-//                   (NCCL exchange), or -- fused exchange -- straight into the owner rank's inbox through
-//                   a peer mapping (NVLink stores).
+//                   flushed in bulk: straight into the set by the warp itself (kmc_run, one rank: K2's
+//                   insert path runs inside K1, see Params::fused), into the local candidate buffer (the
+//                   shard calls at world 1), into per-owner regions (NCCL exchange), or -- fused
+//                   exchange -- straight into the owner rank's inbox through a peer mapping (NVLink stores).
 //   k_insert  (K2)  one thread per candidate: identity (see state_ident), open-addressing hash set in HBM
 //                   with 32-byte buckets (one DRAM sector), CAS insertion, warp ballot/popc compaction of
 //                   the winners into the state store (= next frontier), parent link.  k_insert_inbox is
@@ -198,6 +199,11 @@ struct Params {
   uint64_t inbox_stride;    // words per inbox buffer
   uint32_t p2p;             // 1: expand stores rows straight into the owners' inboxes
   uint32_t inbox_buf;       // which of the two buffers this round uses
+  // 1 (kmc_run, one rank): expand inserts its successors itself (insert_stage) instead of writing them to `cand` for
+  // k_insert.  The kernel then reads the frontier with __ldg while it appends new states to the same store; that is
+  // sound because every new index lies at or beyond the end of the level being expanded, and the
+  // `idx - store_base < max_states` check of insert_row keeps a spilling ring from wrapping onto live states.
+  uint32_t fused;
 };
 
 static constexpr int INBOX_HEADER = 8;
@@ -214,6 +220,9 @@ __device__ __forceinline__ unsigned lane_id() {
   unsigned r;
   asm volatile("mov.u32 %0, %%laneid;" : "=r"(r));
   return r;
+}
+__device__ __forceinline__ void reds_add64(uint32_t a, unsigned long long v) {     // shared-memory add, no return value
+  asm volatile("red.shared.add.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory");
 }
 
 __device__ __noinline__ void record_violation(const Params& p, const State& s, uint64_t meta, uint64_t fp, uint64_t inv) {
@@ -350,8 +359,11 @@ __device__ __forceinline__ Prefetched prefetch_row(const Params& p, const State&
   return f;
 }
 
+// CTA_ACTIONS: the new states per action go to this CTA's shared-memory counters at `act_smem` (u64 per action, the
+// fused expand kernel flushes them once at its end) instead of one global atomic per action and warp.
+template <bool CTA_ACTIONS = false>
 __device__ __forceinline__ void insert_row(const Params& p, const State& s, uint64_t meta, bool valid, const Prefetched& f,
-                                            unsigned& probes, unsigned& oom, int& failed) {
+                                            unsigned& probes, unsigned& oom, int& failed, uint32_t act_smem = 0) {
   bool is_new = false;
   if (valid) {
     if (f.inmodel) {
@@ -380,8 +392,10 @@ __device__ __forceinline__ void insert_row(const Params& p, const State& s, uint
       // none); one atomic per action present among the warp's winners
       const unsigned act = ((meta & 0x0000FFFFFFFFFFFFull) == NO_PARENT) ? ~0u : (unsigned)(meta >> 56);
       const unsigned same = __match_any_sync(mask, act);
-      if (act < (unsigned)M::NUM_ACTIONS && (int)lane == __ffs(same) - 1)
-        atomicAdd(&p.ctr->action_distinct[act], (unsigned long long)__popc(same));
+      if (act < (unsigned)M::NUM_ACTIONS && (int)lane == __ffs(same) - 1) {
+        if (CTA_ACTIONS) reds_add64(act_smem + act * 8, (unsigned long long)__popc(same));
+        else atomicAdd(&p.ctr->action_distinct[act], (unsigned long long)__popc(same));
+      }
       uint64_t idx = base + __popc(mask & ((1u << lane) - 1));
       if (idx - p.store_base < p.max_states) {
         uint64_t* dst = p.store + (idx & p.store_mask) * W;
@@ -449,15 +463,51 @@ __device__ __forceinline__ void claim_and_store(const Params& p, const State& s,
   row[W] = meta;
 }
 
+// Per-CTA counters of the fused insert, u64 each in shared memory, flushed with one global atomic each at the end of
+// k_expand: probes, out-of-model successors, successors generated (the candidate-region check) and new states per action.
+static constexpr int CTA_PROBES = 0, CTA_OOM = 1, CTA_GEN = 2, CTA_ACTION = 3;
+static constexpr int CTA_CTR_BYTES = (CTA_ACTION + M::NUM_ACTIONS) * 8;
+
+// Fused expand + insert (p.fused): the warp inserts its staged rows itself, one row per lane and round, through the
+// insert path of k_insert -- constraint and out-of-model invariant check, identity, probe + CAS, ballot compaction
+// into the store, parent word.  Out of line, so that it exists once in k_expand instead of once per site group and
+// its registers are not live across the bodies.  Called by all 32 lanes of a warp (n is warp-uniform).
+__device__ __noinline__ int insert_stage(const Params& p, uint32_t wbuf, unsigned n, uint32_t cta) {
+  unsigned probes = 0, oom = 0;
+  int failed = 0;
+  const unsigned lane = lane_id();
+  for (unsigned r0 = 0; r0 < n; r0 += 32) {
+    const unsigned r = r0 + lane;
+    const bool valid = r < n;
+    const uint32_t row = wbuf + (valid ? r : 0) * (ROW * 8);
+    State s;
+#pragma unroll
+    for (int k = 0; k < W; ++k) s.w[k] = lds64(row + k * 8);
+    const uint64_t meta = lds64(row + W * 8);
+    const Prefetched f = prefetch_row(p, s, valid);
+    insert_row<true>(p, s, meta, valid, f, probes, oom, failed, cta + CTA_ACTION * 8);
+  }
+  probes = __reduce_add_sync(0xffffffffu, probes);
+  oom = __reduce_add_sync(0xffffffffu, oom);
+  if (lane == 0) {
+    if (probes) reds_add64(cta + CTA_PROBES * 8, probes);
+    if (oom) reds_add64(cta + CTA_OOM * 8, oom);
+  }
+  return failed;
+}
+
 // called by all 32 lanes of a warp at a converged point
-__device__ __forceinline__ void flush_stage(const Params& p, uint32_t wbuf, uint32_t wcnt, bool force, int& failed) {
+__device__ __forceinline__ void flush_stage(const Params& p, uint32_t wbuf, uint32_t wcnt, uint32_t cta, bool force, int& failed) {
   __syncwarp();
   unsigned n;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(n) : "r"(wcnt));
   if (n > (unsigned)STAGE_ROWS) n = STAGE_ROWS;
   if (n == 0 || (!force && n < (unsigned)STAGE_FLUSH)) return;
   unsigned lane = lane_id();
-  if (p.world == 1) {
+  if (p.fused) {
+    const int f = insert_stage(p, wbuf, n, cta);
+    if (f) failed = f;
+  } else if (p.world == 1) {
     unsigned long long base = 0;
     if (lane == 0) base = atomicAdd(&p.ctr->cand_count[0], (unsigned long long)n);
     base = __shfl_sync(0xffffffffu, base, 0);
@@ -546,10 +596,11 @@ static constexpr int SPT = SPT_FIT > 4 ? 4 : SPT_FIT;
 static_assert(SPT >= 1, "state too wide for the expand kernel's shared-memory tile");
 static constexpr int TILE = EXPAND_BLOCK * SPT;
 static_assert(TILE <= LIST_CAP, "a site's segment (<= TILE pairs) must fit one scatter round");
-// the per-site coverage counters live in the slack the tile leaves (SPT is sized without them)
+// the per-site coverage counters and the fused insert's counters live in the slack the tile leaves (SPT is sized
+// without them)
 static constexpr int SITE_GEN_BYTES = (M::NUM_SITES > 0 ? M::NUM_SITES : 1) * 8;
-static constexpr size_t EXPAND_SMEM_BYTES = (size_t)TILE * W * 8 + FIXED_SMEM_BYTES + SITE_GEN_BYTES;
-static_assert(EXPAND_SMEM_BYTES <= 227 * 1024 - 1024, "the per-site coverage counters do not fit next to the expand tile");
+static constexpr size_t EXPAND_SMEM_BYTES = (size_t)TILE * W * 8 + FIXED_SMEM_BYTES + SITE_GEN_BYTES + CTA_CTR_BYTES;
+static_assert(EXPAND_SMEM_BYTES <= 227 * 1024 - 1024, "the per-CTA counters do not fit next to the expand tile");
 
 struct TileCtx {
   uint32_t tile;        // [TILE][W] states (shared-window addresses throughout)
@@ -558,6 +609,7 @@ struct TileCtx {
   uint32_t cur;         // [MAX_GROUP_SITES] scatter cursors
   uint32_t seg;         // [MAX_GROUP_SITES] first chunk of each site's segment
   uint32_t site_gen;    // [NUM_SITES] u64: successors this CTA generated per emit site
+  uint32_t cta;         // the fused insert's counters (CTA_PROBES ...)
   uint32_t wbuf, wcnt;
   uint64_t first, tile_base;
   unsigned nvalid;      // states in this tile
@@ -719,7 +771,7 @@ struct SiteGroupRunner {
           SiteDispatch<BEGIN, END>::run(k + BEGIN, s, sink);
           failed |= sink.failed;
         }
-        flush_stage(p, c.wbuf, c.wcnt, false, failed);
+        flush_stage(p, c.wbuf, c.wcnt, c.cta, false, failed);
       }
       r0 = r_end;
     } while (r0 < total_chunks);
@@ -732,7 +784,8 @@ struct SiteGroupRunner<M::NUM_SITE_GROUPS> {
 };
 
 __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t first, uint64_t count, unsigned tile_states) {
-  extern __shared__ __align__(16) uint64_t smem[];   // tile | stage | list | cnt[2][64] | cur[64] | seg[64] | wcnt[NWARPS] | - | site_gen
+  // tile | stage | list | cnt[2][64] | cur[64] | seg[64] | wcnt[NWARPS] | - | site_gen | CTA counters
+  extern __shared__ __align__(16) uint64_t smem[];
   const int warp = threadIdx.x >> 5;
   TileCtx c;
   c.tile = smem_addr(smem);
@@ -744,9 +797,11 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
   c.seg = c.cur + MAX_GROUP_SITES * 4;
   c.wcnt = c.seg + MAX_GROUP_SITES * 4 + warp * 4;
   c.site_gen = c.seg + MAX_GROUP_SITES * 4 + (NWARPS + 8) * 4;
+  c.cta = c.site_gen + SITE_GEN_BYTES;
   c.first = first;
   if (lane_id() == 0) sts32(c.wcnt, 0u);
   for (unsigned i = threadIdx.x; i < (unsigned)M::NUM_SITES; i += EXPAND_BLOCK) sts64(c.site_gen + i * 8, 0ull);
+  for (unsigned i = threadIdx.x; i < (unsigned)(CTA_CTR_BYTES / 8); i += EXPAND_BLOCK) sts64(c.cta + i * 8, 0ull);
   unsigned long long gen = 0, dead = 0;
   unsigned maxfan = 0;
   int failed = 0;
@@ -775,7 +830,7 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
 #pragma unroll
     for (int j = 0; j < SPT; ++j) nsucc[j] = 0;
     SiteGroupRunner<0>::run(p, c, nsucc, failed);
-    flush_stage(p, c.wbuf, c.wcnt, true, failed);
+    flush_stage(p, c.wbuf, c.wcnt, c.cta, true, failed);
 #pragma unroll
     for (int j = 0; j < SPT; ++j) {
       const unsigned slot = (unsigned)j * EXPAND_BLOCK + threadIdx.x;
@@ -794,12 +849,6 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
       }
     }
   }
-  // coverage: one atomic per (CTA, site)
-  __syncthreads();
-  for (unsigned i = threadIdx.x; i < (unsigned)M::NUM_SITES; i += EXPAND_BLOCK) {
-    const unsigned long long v = lds64(c.site_gen + i * 8);
-    if (v) atomicAdd(&p.ctr->site_generated[i], v);
-  }
   // warp reduce the statistics, one atomic per warp
   for (int o = 16; o > 0; o >>= 1) {
     gen += __shfl_xor_sync(0xffffffffu, gen, o);
@@ -812,6 +861,29 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
     if (dead) atomicAdd(&p.ctr->deadlocks, dead);
     if (maxfan) atomicMax(&p.ctr->max_fanout_seen, (unsigned long long)maxfan);
     if (failed) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)failed);
+    if (p.fused && gen) reds_add64(c.cta + CTA_GEN * 8, gen);
+  }
+  // coverage and the fused insert's counters: one atomic per (CTA, counter)
+  __syncthreads();
+  for (unsigned i = threadIdx.x; i < (unsigned)M::NUM_SITES; i += EXPAND_BLOCK) {
+    const unsigned long long v = lds64(c.site_gen + i * 8);
+    if (v) atomicAdd(&p.ctr->site_generated[i], v);
+  }
+  if (p.fused) {
+    for (unsigned i = threadIdx.x; i < (unsigned)M::NUM_ACTIONS; i += EXPAND_BLOCK) {
+      const unsigned long long v = lds64(c.cta + (CTA_ACTION + i) * 8);
+      if (v) atomicAdd(&p.ctr->action_distinct[i], v);
+    }
+    if (threadIdx.x == 0) {
+      const unsigned long long probes = lds64(c.cta + CTA_PROBES * 8), oom = lds64(c.cta + CTA_OOM * 8);
+      if (probes) atomicAdd(&p.ctr->probes, probes);
+      if (oom) atomicAdd(&p.ctr->out_of_model, oom);
+      // No candidate rows are written, but a chunk's successors are still bounded by the candidate region, so that
+      // cand_bytes and fanout_bound mean the same with and without fusion: the CTA whose total crosses it fails the run.
+      const unsigned long long g = lds64(c.cta + CTA_GEN * 8);
+      if (g && atomicAdd(&p.ctr->cand_count[0], g) + g > p.region_rows)
+        atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)KMC_FAIL_CAND_FULL);
+    }
   }
 }
 
@@ -1153,6 +1225,7 @@ struct Engine {
     p.inbox_stride = inbox_stride;
     p.p2p = 0;
     p.inbox_buf = inbox_buf;
+    p.fused = 0;
     return p;
   }
 };
@@ -1439,9 +1512,12 @@ static int launch_invariants(Engine& E, uint64_t first, uint64_t count_bound) {
   return KMC_OK;
 }
 
-static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false) {
+// fused (kmc_run, one rank): the kernel inserts the successors itself; otherwise they go to the candidate buffer
+// (or the owners' inboxes) for k_insert / k_insert_inbox
+static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false, bool fused = false) {
   Params p = E.params();
   p.p2p = p2p ? 1 : 0;
+  p.fused = fused ? 1 : 0;
   if (count == 0) return KMC_OK;
   TimedLaunch t(E, 0);
   // small levels: smaller tiles so that every SM still gets one (a tile is a multiple of 32 states)
@@ -1761,9 +1837,10 @@ static int engine_run(Engine& E) {
     const uint64_t level_end = E.level_first + E.level_count;
     for (uint64_t off = E.level_first, slot, cnt; off < level_end; off += cnt) {
       cnt = std::min<uint64_t>(E.chunk_states, ring_run(E, off, level_end, &slot));   // a chunk never crosses the wrap
+      // one launch per chunk: the expand kernel inserts its successors itself (Params::fused); the candidate
+      // counter only bounds the chunk's successors
       if ((rc = reset_cand(E))) return rc;
-      if ((rc = launch_expand(E, off, cnt))) return rc;
-      if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, cnt * (uint64_t)E.fanout_bound))) return rc;
+      if ((rc = launch_expand(E, off, cnt, false, true))) return rc;
     }
     if ((rc = end_level(E, E.level_count * 2, false, h))) return rc;
     err = fail_to_error(h.fail);
