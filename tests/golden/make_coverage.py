@@ -7,7 +7,7 @@ full BFS (past violations, like -continue), the numbers a GPU run's coverage rep
     interpreter finishes in seconds; elsewhere the lowered model's own labels, counted by the sequential host
     harness (tests/support/hostmodel.run_host);
   * per site: Oracle A has no emit sites, so these come from the lowered header on the host: the popcount of each
-    site_mask bit over the states the host BFS expands (tests/support/host_coverage.py).  Under SYMMETRY these
+    site_mask bit over the states the host BFS expands (tests/support/hostmodel.site_coverage).  Under SYMMETRY these
     depend on which member of each orbit is stored (the first one found here, the insert's winner on the GPU), so
     they are exact only for models without it; per action they are the same either way.
 
@@ -34,8 +34,7 @@ ORACLE_A = ["idsequence", "idsequence_deadlock", "frl_tiny", "kip320_n2", "trunc
 def one(name: str, spec: dict) -> tuple[str, dict]:
     from kafka_specification_b200.build import tla_search_dirs
     from kafka_specification_b200.lower.model import lower_model
-    from host_coverage import site_coverage
-    from hostmodel import run_host
+    from hostmodel import run_host, site_coverage
     cfg_text = open(os.path.join(ROOT, spec["cfg"])).read()
     model = lower_model(spec["module"], tla_search_dirs(), cfg_text, name=name)
     names = [a["name"] for a in model.actions]

@@ -1,55 +1,18 @@
-"""CPU stand-in for one rank of the sharded engine (tests only), see host_shard.cpp."""
+"""CPU stand-in for one rank of the sharded engine (tests only), see the hs_* calls of host_model.cpp."""
 from __future__ import annotations
 
 import ctypes
-import hashlib
-import os
-import subprocess
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-
-
-def build(name: str) -> ctypes.CDLL:
-    hdr = os.path.join(ROOT, "build", "models", name, "model.h")
-    tag = hashlib.sha256(open(hdr, "rb").read() + open(os.path.join(HERE, "host_shard.cpp"), "rb").read()).hexdigest()[:12]
-    out = os.path.join(ROOT, "build", "hosttest")
-    os.makedirs(out, exist_ok=True)
-    so = os.path.join(out, f"shard_{name}_{tag}.so")
-    if not os.path.exists(so):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", f'-DKMC_MODEL_HEADER="{hdr}"',
-                               os.path.join(HERE, "host_shard.cpp"), "-o", tmp])
-        os.replace(tmp, so)
-    lib = ctypes.CDLL(so)
-    lib.hs_create.restype = ctypes.c_void_p
-    lib.hs_create.argtypes = [ctypes.c_uint32, ctypes.c_uint32]
-    for fn in ("hs_destroy", "hs_begin", "hs_seed_init", "hs_reset_cand"):
-        getattr(lib, fn).argtypes = [ctypes.c_void_p]
-        getattr(lib, fn).restype = None
-    lib.hs_expand.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint64]
-    lib.hs_expand.restype = None
-    lib.hs_counts.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    lib.hs_counts.restype = None
-    lib.hs_send_ptr.argtypes = [ctypes.c_void_p, ctypes.c_uint32]
-    lib.hs_send_ptr.restype = ctypes.POINTER(ctypes.c_int64)
-    lib.hs_recv_ptr.argtypes = [ctypes.c_void_p, ctypes.c_uint64]
-    lib.hs_recv_ptr.restype = ctypes.POINTER(ctypes.c_int64)
-    lib.hs_insert.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64]
-    lib.hs_insert.restype = None
-    lib.hs_level_done.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    lib.hs_level_done.restype = None
-    lib.hs_stats.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    lib.hs_stats.restype = None
-    return lib
+from hostmodel import HostModel
 
 
 class HostShardEngine:
     def __init__(self, name: str, rank: int, world: int, chunk_states: int = 1000):
-        self.lib = build(name)
+        self.model = HostModel.for_built_model(name)
+        self.lib = self.model.lib
         self.rank, self.world = rank, world
         self.h = self.lib.hs_create(rank, world)
         self.row_words = self.lib.hs_row_words()
@@ -119,7 +82,6 @@ class HostShardEngine:
 
     def _record(self):
         out = np.zeros(self.row_words + 4, dtype=np.uint64)
-        self.lib.hs_violation_record.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
         inv = self.lib.hs_violation_record(self.h, out.ctypes.data)
         return inv, out
 
@@ -139,16 +101,14 @@ class HostShardEngine:
 
     def state_and_parent(self, idx):
         out = np.zeros(self.row_words, dtype=np.uint64)
-        self.lib.hs_state_and_parent.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]
         self.lib.hs_state_and_parent(self.h, idx, out.ctypes.data)
         return [int(x) for x in out[:-1]], int(out[-1])
 
     def is_successor(self, a, b) -> int:
-        self.lib.hs_is_successor.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-        x, y = np.array(a, dtype=np.uint64), np.array(b, dtype=np.uint64)
-        return self.lib.hs_is_successor(x.ctypes.data, y.ctypes.data)
+        """The action id of a successor of state a under expand() equal to b, or -1."""
+        rows, actions = self.model.successors(a)
+        hit = np.flatnonzero(np.all(rows == np.asarray(b, dtype=np.uint64), axis=1))
+        return int(actions[hit[0]]) if len(hit) else -1
 
     def is_init(self, a) -> int:
-        self.lib.hs_is_init.argtypes = [ctypes.c_void_p]
-        x = np.array(a, dtype=np.uint64)
-        return self.lib.hs_is_init(x.ctypes.data)
+        return int(bool(np.all(self.model.init_states() == np.asarray(a, dtype=np.uint64), axis=1).any()))

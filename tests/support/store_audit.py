@@ -1,8 +1,8 @@
-"""Test support: the whole-store audit of a GPU run (host_audit.cpp) and a reference of the engine's fingerprints.
+"""Test support: the whole-store audit of a GPU run (host_model.cpp) and a reference of the engine's fingerprints.
 
 ``audit_checker(ck, levels, distinct)`` reads every stored state and parent word of a finished or stopped run and checks them
 against the lowered Next compiled for the host from the same ``model.h`` (init, edges, uniqueness, closure; see
-host_audit.cpp), then compares the totals the audit recomputes from the stored states with the run's stats and
+audit_store in host_model.cpp), then compares the totals the audit recomputes from the stored states with the run's stats and
 coverage, and the reported counterexample with the one ``build_trace``'s rule picks among the violators the engine
 records: deadlocks first, then the smallest fingerprint, then the smallest parent word.
 
@@ -12,14 +12,10 @@ key_of, bucket_of, owner_of), once over NumPy arrays and once over Python ints.
 from __future__ import annotations
 
 import ctypes
-import hashlib
-import json
-import os
-import subprocess
 
 import numpy as np
 
-from hostmodel import BUILD, HERE, ROOT
+from hostmodel import HostModel
 
 NO_PARENT = 0x0000FFFFFFFFFFFF
 VIOL_RING = 1 << 16          # rows of the engine's violator ring; past it the reported pick is not deterministic
@@ -133,62 +129,8 @@ def owner_of(fp: np.ndarray, world: int) -> np.ndarray:
 
 
 # ------------------------------------------------------------------------------------------------ the host library
-class AuditLib:
-    """host_audit.cpp compiled against one model header."""
-
-    def __init__(self, name: str, header_text: str):
-        os.makedirs(BUILD, exist_ok=True)
-        src = os.path.join(HERE, "host_audit.cpp")
-        tag = hashlib.sha256((header_text + open(src).read()).encode()).hexdigest()[:16]
-        hdr = os.path.join(BUILD, f"audit_{name}_{tag}.h")
-        so = os.path.join(BUILD, f"audit_{name}_{tag}.so")
-        if not os.path.exists(so):
-            with open(hdr, "w") as f:
-                f.write(header_text)
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", f'-DKMC_MODEL_HEADER="{hdr}"', src,
-                                   "-o", so + ".tmp"])
-            os.replace(so + ".tmp", so)
-        lib = ctypes.CDLL(so)
-        vp = ctypes.c_void_p
-        lib.audit_digest.restype = ctypes.c_char_p
-        lib.audit_canonicalize.argtypes = [vp, ctypes.c_uint64, vp]
-        lib.audit_canonicalize.restype = None
-        lib.audit_store.argtypes = [vp, vp, vp, ctypes.c_uint64, vp, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int,
-                                    vp, vp, vp, vp, ctypes.c_char_p, ctypes.c_size_t]
-        lib.audit_violator_rows.argtypes = [vp, ctypes.c_uint64]
-        lib.audit_violator_rows.restype = ctypes.c_uint64
-        lib.audit_host_bfs.argtypes = [vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, ctypes.c_uint32, vp, vp]
-        lib.audit_host_bfs.restype = ctypes.c_int64
-        self.lib = lib
-        self.name = name
-        self.words = lib.audit_words()
-        self.state_bits = lib.audit_state_bits()
-        self.all_ones_possible = bool(lib.audit_all_ones_possible())
-        self.symmetry = bool(lib.audit_has_symmetry())
-        self.num_actions = lib.audit_num_actions()
-        self.num_sites = lib.audit_num_sites()
-        self.num_init = lib.audit_num_init()
-        self.check_deadlock = bool(lib.audit_check_deadlock())
-        self.digest = lib.audit_digest().decode()
-
-    @classmethod
-    def for_built_model(cls, name: str) -> "AuditLib":
-        """The audit of build/models/<name>/model.h, the header libkmc_<name>.so was compiled from."""
-        d = os.path.join(ROOT, "build", "models", name)
-        with open(os.path.join(d, "model.h")) as f:
-            a = cls(name, f.read())
-        with open(os.path.join(d, "model.json")) as f:
-            digest = json.load(f)["digest"]
-        if a.digest != digest:
-            raise AuditError(f"digest: model.h ({a.digest}) and model.json ({digest}) of {name} disagree")
-        return a
-
-    def canonicalize(self, rows: np.ndarray) -> np.ndarray:
-        rows = np.ascontiguousarray(rows, dtype=np.uint64).reshape(-1, self.words)
-        out = np.empty_like(rows)
-        if len(rows):
-            self.lib.audit_canonicalize(rows.ctypes.data, len(rows), out.ctypes.data)
-        return out
+class AuditLib(HostModel):
+    """host_model.cpp compiled against one model header, with the audit's entry points."""
 
     def fingerprints(self, rows: np.ndarray, canonical: np.ndarray | bool = False) -> np.ndarray:
         """The engine's fingerprint of each row, of its canonical form where `canonical` says so."""
@@ -199,18 +141,14 @@ class AuditLib:
             src[canonical] = self.canonicalize(rows[canonical])
         return fingerprint(src, self.state_bits)
 
-    def host_bfs(self, stop_after: int = 0, cap: int = 4_000_000) -> dict:
-        """Level-ordered host BFS that writes its store in the engine's format (no constraint on which orbit member)."""
-        states = np.zeros((cap, self.words), dtype=np.uint64)
-        parents = np.zeros(cap, dtype=np.uint64)
-        widths = np.zeros(4096, dtype=np.uint64)
-        n_levels, n_exp = ctypes.c_uint32(), ctypes.c_uint32()
-        n = self.lib.audit_host_bfs(states.ctypes.data, parents.ctypes.data, cap, stop_after, widths.ctypes.data, 4096,
-                                    ctypes.byref(n_levels), ctypes.byref(n_exp))
-        if n < 0:
-            raise RuntimeError(f"{self.name}: host BFS exceeded {cap} states or trapped the layout")
-        return {"states": states[:n].copy(), "parents": parents[:n].copy(),
-                "widths": [int(x) for x in widths[: n_levels.value]], "n_expanded": n_exp.value}
+    def host_bfs(self, stop_after: int = 0, sites: bool = False) -> dict:
+        """Level-ordered host BFS that writes its store in the engine's format, through expand() or, with `sites`, the
+        two-phase form (which orbit member is stored follows the order of the form); stops at the first level end that
+        holds >= stop_after states (0: never)."""
+        r = self.bfs(sites=sites, stop_at=stop_after)
+        if r["fail"]:
+            raise RuntimeError(f"{self.name}: host BFS trapped the layout (code {r['fail']})")
+        return {"states": r["states"], "parents": r["parents"], "widths": r["widths"], "n_expanded": r["n_expanded"]}
 
     def check_store(self, states, parents, widths, n_expanded: int, *, check_deadlock: bool,
                     rank_widths: list[list[int]] | None = None) -> dict:

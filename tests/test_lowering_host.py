@@ -1,7 +1,7 @@
 """The AOT lowering, compiled for the HOST by the test harness, against the goldens.
 
 This exercises exactly the header the CUDA engine includes (same expand / invariant / constraint
-code, same packed layout) on a machine without a GPU.  The harness (tests/support/host_bfs.cpp)
+code, same packed layout) on a machine without a GPU.  The harness (tests/support/host_model.cpp)
 is test infrastructure: no product path runs on the CPU.
 """
 import os

@@ -12,7 +12,6 @@ between Oracle A (evaluating the reference's text for this cfg) and the lowered 
 compiles), in both forms of the lowered Next.  Every state visited is reachable by construction as long as all earlier
 steps agreed -- and the first disagreement fails the test.  Walks are long enough to reach the deep levels (full logs,
 maximal epochs) that a bounded BFS prefix never sees."""
-import ctypes
 import os
 import random
 
@@ -20,7 +19,7 @@ import numpy as np
 import pytest
 
 from conftest import REFERENCE, ROOT, needs_reference
-from hostmodel import build_host, lower_model
+from hostmodel import HostModel, lower_model
 
 DIRS = [REFERENCE, os.path.join(ROOT, "models"), os.path.join(ROOT, "tests", "specs")]
 
@@ -43,12 +42,7 @@ def test_random_walks_agree_with_oracle_a_step_by_step(name, walks, steps, regis
     spec = registry[name]
     cfg_text = open(os.path.join(ROOT, spec["cfg"])).read()
     m = lower_model(spec["module"], DIRS, cfg_text, name=name)
-    lib = build_host(m)
-    W = m.words
-    lib.kmc_host_successors.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
-    lib.kmc_host_first_violated.argtypes = [ctypes.c_void_p]
-    lib.kmc_host_in_model.argtypes = [ctypes.c_void_p]
-    lib.kmc_host_init_state.argtypes = [ctypes.c_int, ctypes.c_void_p]
+    hm = HostModel.from_lowered(m)
 
     cfg = parse_cfg(cfg_text)
     root = load_root(spec["module"], DIRS)
@@ -59,11 +53,7 @@ def test_random_walks_agree_with_oracle_a_step_by_step(name, walks, steps, regis
 
     # Init: the same set of states on both sides
     a_inits = sorted(_text(variables, st) for st in it.init_states(init_e))
-    l_inits = []
-    for i in range(lib.kmc_host_num_init()):
-        w = np.zeros(W, dtype=np.uint64)
-        lib.kmc_host_init_state(i, w.ctypes.data)
-        l_inits.append(w)
+    l_inits = list(hm.init_states())
     assert sorted(m.state_text(w) for w in l_inits) == a_inits
 
     walks *= int(os.environ.get("KSPEC_WALK_SCALE", "1"))          # (a longer offline run: KSPEC_WALK_SCALE=10)
@@ -73,8 +63,6 @@ def test_random_walks_agree_with_oracle_a_step_by_step(name, walks, steps, regis
         kafka_b = tuple(spec["kso"])
         replicas = sorted(m.decode_state(l_inits[0])["replicaLog"].domain(), key=str)
     rng = random.Random(20260923 + len(name))
-    cap = max(512, 4 * m.max_fanout)
-    out = np.zeros((cap, W), dtype=np.uint64)
     compared = deepest = 0
     for _ in range(walks):
         cur = l_inits[rng.randrange(len(l_inits))].copy()
@@ -83,9 +71,9 @@ def test_random_walks_agree_with_oracle_a_step_by_step(name, walks, steps, regis
             assert m.lowerer.layout.py_pack(st) == [int(x) for x in cur]        # decode/encode round trip
             # verdicts
             viol_a = next((i for i, inv in enumerate(cfg.invariants) if not it.eval_named_predicate(inv, st)), -1)
-            assert lib.kmc_host_first_violated(cur.ctypes.data) == viol_a, (name, step, m.state_text(cur))
+            assert hm.first_violated(cur) == viol_a, (name, step, m.state_text(cur))
             inmodel_a = all(it.eval_named_predicate(c, st) for c in cfg.constraints)
-            assert bool(lib.kmc_host_in_model(cur.ctypes.data)) == inmodel_a
+            assert hm.in_model(cur) == inmodel_a
             # successors: multiset of canonical texts, both forms of the lowered Next
             succ_a = it.next_states(next_e, st)
             want = sorted(_text(variables, s1) for s1 in succ_a)
@@ -100,15 +88,13 @@ def test_random_walks_agree_with_oracle_a_step_by_step(name, walks, steps, regis
                 assert set(kso.violated(model_b, params_b, rec, inv_b)) == {i for i in inv_b if not it.eval_named_predicate(i, st)}
             rows = None
             for items in (0, 1):
-                n = lib.kmc_host_successors(cur.ctypes.data, items, out.ctypes.data, None, cap)
-                assert 0 <= n <= cap, (name, "layout trap or fan-out above the buffer", n)
-                got = sorted(m.state_text(out[k]) for k in range(n))
+                rows, _ = hm.successors(cur, sites=bool(items))          # (a layout trap raises)
+                got = sorted(m.state_text(r) for r in rows)
                 assert got == want, (name, f"step {step}, form {items}: successors differ for\n{m.state_text(cur)}")
-                rows = out[:n].copy()
             compared += 1
             deepest = max(deepest, step + 1)
             # continue from a random in-model successor (out-of-model ones are not expanded by a checker)
-            nxt = [r for r in rows if lib.kmc_host_in_model(r.ctypes.data)]
+            nxt = [r for r in rows if hm.in_model(r)]
             if not nxt:
                 break
             cur = nxt[rng.randrange(len(nxt))].copy()
@@ -128,25 +114,15 @@ def test_canonicalize_is_an_orbit_invariant_on_deep_states(name, walks, steps, r
     spec = registry[name]
     cfg_text = open(os.path.join(ROOT, spec["cfg"])).read()
     m = lower_model(spec["module"], DIRS, cfg_text, name=name)
-    lib = build_host(m)
-    W = m.words
-    lib.kmc_host_successors.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
-    lib.kmc_host_canonicalize.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    lib.kmc_host_init_state.argtypes = [ctypes.c_int, ctypes.c_void_p]
-    lib.kmc_host_in_model.argtypes = [ctypes.c_void_p]
+    hm = HostModel.from_lowered(m)
     lay = m.lowerer.layout
     replicas = sorted(m.decode_state(np.array(m.init_states[0], dtype=np.uint64))["replicaLog"].domain(), key=str)
     perms = [dict(zip(replicas, p)) for p in itertools.permutations(replicas)]
 
     def canon(words):
-        w = np.array(words, dtype=np.uint64)
-        out = np.zeros(W, dtype=np.uint64)
-        lib.kmc_host_canonicalize(w.ctypes.data, out.ctypes.data)
-        return tuple(int(x) for x in out)
+        return tuple(int(x) for x in hm.canonicalize(np.array(words, dtype=np.uint64))[0])
 
     rng = random.Random(7 + len(name))
-    cap = max(512, 4 * m.max_fanout)
-    out = np.zeros((cap, W), dtype=np.uint64)
     checked = 0
     for _ in range(walks):
         cur = np.array(m.init_states[0], dtype=np.uint64)
@@ -161,9 +137,8 @@ def test_canonicalize_is_an_orbit_invariant_on_deep_states(name, walks, steps, r
                 assert canon(words) == c0, (name, step, pm)
             assert c0 in images and canon(c0) == c0
             checked += 1
-            n = lib.kmc_host_successors(cur.ctypes.data, 0, out.ctypes.data, None, cap)
-            assert 0 < n <= cap or n == 0
-            if n == 0:
+            out, _ = hm.successors(cur)                               # (a layout trap raises)
+            if len(out) == 0:
                 break
-            cur = out[rng.randrange(n)].copy()
+            cur = out[rng.randrange(len(out))].copy()
     assert checked >= walks * 10

@@ -1,6 +1,6 @@
-"""The whole-store audit (tests/support/host_audit.cpp, store_audit.py) on the CPU: it accepts a clean store written in
-the engine's format by a level-ordered host BFS, and rejects each kind of corruption with the check that catches it.
-The reference fingerprints are checked against their pure-int restatement."""
+"""The whole-store audit (tests/support/host_model.cpp, store_audit.py) on the CPU: it accepts a clean store written in
+the engine's format by a level-ordered host BFS through the two-phase form, and rejects each kind of corruption with
+the check that catches it.  The reference fingerprints are checked against their pure-int restatement."""
 import os
 
 import numpy as np
@@ -25,7 +25,7 @@ def clean_stores(registry):
     out = {}
     for name in AUDITED:
         a = _audit_lib(registry, name)
-        out[name] = (a, a.host_bfs())
+        out[name] = (a, a.host_bfs(sites=True))     # the order coverage.json was made in
     return out
 
 
@@ -42,7 +42,7 @@ def _check(a, st, goldens, coverage_golden=None, deadlocks=None):
         init = (parents & np.uint64(0xFFFFFFFFFFFF)) == np.uint64(0xFFFFFFFFFFFF)
         hist = np.bincount((parents[~init] >> np.uint64(56)).astype(np.int64), minlength=a.num_actions)
         cov = {"actions": [{"generated": c["per_action"][n], "distinct": int(hist[i])} for i, n in enumerate(c["actions"])],
-               "sites": found["site_generated"] if a.symmetry else c["per_site"]}
+               "sites": c["per_site"]}
     compare(a, found, stats=stats, coverage=cov, parents=st["parents"], violation=None, record=None, invariants=[])
     return found
 

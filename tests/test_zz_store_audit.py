@@ -1,5 +1,5 @@
 """Whole-store audits of GPU runs: every stored state, parent word and counterexample against the lowered Next compiled
-for the host (tests/support/host_audit.cpp, store_audit.py).  The totals and digests of the other GPU tests cannot see
+for the host (tests/support/host_model.cpp, store_audit.py).  The totals and digests of the other GPU tests cannot see
 an off-by-one tile offset, a scatter round labelling pairs with the wrong tile slot, a chunk or ring offset error, or
 two actions of equal fan-out swapping ids: each of these keeps every count and corrupts traces and coverage.  The
 audit checks, for each state, that its parent word names a state of the previous level whose Next produces exactly
@@ -120,7 +120,7 @@ def test_store_audit_four_words_bounded(goldens):
     no golden: the bounded run's levels equal the host BFS's, and the audit needs no golden."""
     from store_audit import AuditLib
     a = AuditLib.for_built_model("kip320_5brokers")
-    host = a.host_bfs(stop_after=800_000, cap=2_000_000)
+    host = a.host_bfs(stop_after=800_000)
     assert a.words == 4 and a.num_sites == 259
     r, rep = audit_run("kip320_5brokers", stop_after_states=800_000, max_states=1 << 21)
     assert rep["widths"] == host["widths"] and len(r.levels) == host["n_expanded"]
