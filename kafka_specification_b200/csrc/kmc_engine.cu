@@ -225,10 +225,13 @@ __device__ __forceinline__ void reds_add64(uint32_t a, unsigned long long v) {  
   asm volatile("red.shared.add.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory");
 }
 
-__device__ __noinline__ void record_violation(const Params& p, const State& s, uint64_t meta, uint64_t fp, uint64_t inv) {
-  unsigned long long slot = atomicAdd(&p.ctr->viol_count, 1ull);
+// Out of line (rare, terminal), so it takes the two pointers it uses by value: a `const Params&` argument would make
+// the caller keep a copy of the kernel parameters in local memory and reach them through generic loads.
+__device__ __noinline__ void record_violation(DevCounters* ctr, uint64_t* viol_ring, const State& s, uint64_t meta, uint64_t fp,
+                                              uint64_t inv) {
+  unsigned long long slot = atomicAdd(&ctr->viol_count, 1ull);
   if (slot >= (unsigned long long)VIOL_RING) return;
-  uint64_t* row = p.viol_ring + slot * VIOL_ROW;
+  uint64_t* row = viol_ring + slot * VIOL_ROW;
 #pragma unroll
   for (int k = 0; k < W; ++k) row[k] = s.w[k];
   row[W] = meta;
@@ -376,7 +379,7 @@ __device__ __forceinline__ void insert_row(const Params& p, const State& s, uint
       // so that (rare) case is handled here.  New in-model states are checked by k_invariants (K3).
       if (M::NUM_INVARIANTS > 0) {
         int inv = M::first_violated_invariant(s);
-        if (inv >= 0) record_violation(p, s, meta, f.id.fp, (uint64_t)inv);
+        if (inv >= 0) record_violation(p.ctr, p.viol_ring, s, meta, f.id.fp, (uint64_t)inv);
       }
     }
   }
@@ -472,7 +475,21 @@ static constexpr int CTA_CTR_BYTES = (CTA_ACTION + M::NUM_ACTIONS) * 8;
 // insert path of k_insert -- constraint and out-of-model invariant check, identity, probe + CAS, ballot compaction
 // into the store, parent word.  Out of line, so that it exists once in k_expand instead of once per site group and
 // its registers are not live across the bodies.  Called by all 32 lanes of a warp (n is warp-uniform).
-__device__ __noinline__ int insert_stage(const Params& p, uint32_t wbuf, unsigned n, uint32_t cta) {
+// It gets the kernel parameters it reads by value, in registers: with a `const Params&` argument the caller kept a copy
+// of Params in local memory and the insert reached every pointer through a generic load ahead of its first probe.
+__device__ __noinline__ int insert_stage(void* table, uint64_t bucket_mask, uint64_t* store, uint64_t* parent,
+                                         uint64_t max_states, uint64_t store_mask, uint64_t store_base, DevCounters* ctr,
+                                         uint64_t* viol_ring, uint32_t wbuf, unsigned n, uint32_t cta) {
+  Params p{};          // a value: only the fields above are read, and it is never addressed
+  p.table = table;
+  p.bucket_mask = bucket_mask;
+  p.store = store;
+  p.parent = parent;
+  p.max_states = max_states;
+  p.store_mask = store_mask;
+  p.store_base = store_base;
+  p.ctr = ctr;
+  p.viol_ring = viol_ring;
   unsigned probes = 0, oom = 0;
   int failed = 0;
   const unsigned lane = lane_id();
@@ -505,7 +522,8 @@ __device__ __forceinline__ void flush_stage(const Params& p, uint32_t wbuf, uint
   if (n == 0 || (!force && n < (unsigned)STAGE_FLUSH)) return;
   unsigned lane = lane_id();
   if (p.fused) {
-    const int f = insert_stage(p, wbuf, n, cta);
+    const int f = insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
+                               p.viol_ring, wbuf, n, cta);
     if (f) failed = f;
   } else if (p.world == 1) {
     unsigned long long base = 0;
@@ -843,7 +861,7 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
             State s;
             const uint64_t gi = (first + tile_base + slot) & p.store_mask;
             load_state(s, p.store + gi * W);
-            record_violation(p, s, p.parent[gi], fingerprint(s), ~0ull);
+            record_violation(p.ctr, p.viol_ring, s, p.parent[gi], fingerprint(s), ~0ull);
           }
         }
       }
@@ -1087,7 +1105,7 @@ __global__ void __launch_bounds__(256) k_invariants(Params p, uint64_t first, co
 #pragma unroll
     for (int k = 0; k < W; ++k) s.w[k] = __ldcs(src + k);
     int inv = M::first_violated_invariant(s);
-    if (inv >= 0) record_violation(p, s, p.parent[i & p.store_mask], fingerprint(s), (uint64_t)inv);
+    if (inv >= 0) record_violation(p.ctr, p.viol_ring, s, p.parent[i & p.store_mask], fingerprint(s), (uint64_t)inv);
   }
 }
 
