@@ -88,7 +88,8 @@ typedef struct {
   int32_t invariant;        /* index into the cfg's INVARIANT list, -1 for deadlock       */
   uint64_t level;           /* BFS level of the offending state (Init = 1)                */
   uint64_t trace_len;       /* number of states in the error trace                        */
-  uint64_t fingerprint;     /* 64-bit fingerprint of the offending state                  */
+  uint64_t fingerprint;     /* 64-bit fingerprint of the offending state; under SYMMETRY that of
+                               its orbit (the canonical form), whichever member was reached  */
 } kmc_violation_t;
 
 typedef struct {

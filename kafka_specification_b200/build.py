@@ -1,6 +1,6 @@
 """Ahead-of-time build: ``.tla`` + ``.cfg``  ->  lowered header  ->  ``libkmc_<model>.so`` (sm_90a).
 
-    python -m kafka_specification_b200.build --all            # every model in models/MODELS.json
+    python -m kafka_specification_b200.build --all            # every model in models/ and tests/specs/MODELS.json
     python -m kafka_specification_b200.build Kip320 models/Kip320.cfg --name kip320
 
 Artifacts go to ``build/`` (git-ignored):
@@ -29,6 +29,7 @@ BUILD = os.path.join(ROOT, "build")
 CSRC = os.path.join(ROOT, "kafka_specification_b200", "csrc")
 INCLUDE = os.path.join(ROOT, "include")
 MODELS_DIR = os.path.join(ROOT, "models")
+TEST_SPECS_DIR = os.path.join(ROOT, "tests", "specs")
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 SPEC_DIR = os.path.join(ROOT, "oracle", "_ref", "spec")
@@ -39,7 +40,7 @@ def tla_search_dirs() -> list[str]:
     env = os.environ.get("KSPEC_TLA_PATH")
     if env:
         dirs += env.split(os.pathsep)
-    dirs += [SPEC_DIR, MODELS_DIR, os.path.join(ROOT, "tests", "specs")]
+    dirs += [SPEC_DIR, MODELS_DIR, TEST_SPECS_DIR]
     return [d for d in dirs if os.path.isdir(d)]
 
 
@@ -159,8 +160,19 @@ def build_model(module: str, cfg_path: str, name: str, force: bool = False) -> s
 
 
 def registry() -> dict:
+    """Every model build_all() compiles: the project's models (models/MODELS.json) and the models that exist only to
+    test the engine (tests/specs/MODELS.json, specs kept with the tests; absent from a tree without the test suite)."""
     with open(os.path.join(MODELS_DIR, "MODELS.json")) as f:
-        return json.load(f)
+        reg = json.load(f)
+    test_registry = os.path.join(TEST_SPECS_DIR, "MODELS.json")
+    if not os.path.exists(test_registry):
+        return reg
+    with open(test_registry) as f:
+        test_models = json.load(f)
+    clash = set(reg) & set(test_models)
+    if clash:
+        raise RuntimeError(f"models registered twice: {sorted(clash)}")
+    return {**reg, **test_models}
 
 
 def build_all(force: bool = False, only: list[str] | None = None, verbose: bool = True, jobs: int = 0) -> dict[str, str]:

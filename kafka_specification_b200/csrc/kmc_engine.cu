@@ -174,7 +174,9 @@ struct DevCounters {
 // Violating states are rare and terminal, so they go to a small ring: W state words, the
 // parent/action word, the fingerprint and the invariant index (~0 = deadlock).  The host picks
 // the entry with the smallest fingerprint -> the reported counterexample is deterministic
-// (as long as the first violating level has <= VIOL_RING violators).
+// (as long as the first violating level has <= VIOL_RING violators).  Every writer fingerprints
+// the violator by its set identity (state_fp: the orbit representative under SYMMETRY), never by
+// the stored orbit member, which is whichever insert won: the pick is then a choice among orbits.
 static constexpr int VIOL_RING = 1 << 16;     // rows; (W + 3) * 8 bytes each: 2.6 MB for a two-word model
 static constexpr int VIOL_ROW = W + 3;
 
@@ -861,7 +863,7 @@ __global__ void __launch_bounds__(EXPAND_BLOCK, 1) k_expand(Params p, uint64_t f
             State s;
             const uint64_t gi = (first + tile_base + slot) & p.store_mask;
             load_state(s, p.store + gi * W);
-            record_violation(p.ctr, p.viol_ring, s, p.parent[gi], fingerprint(s), ~0ull);
+            record_violation(p.ctr, p.viol_ring, s, p.parent[gi], state_fp(s), ~0ull);
           }
         }
       }
@@ -1105,7 +1107,7 @@ __global__ void __launch_bounds__(256) k_invariants(Params p, uint64_t first, co
 #pragma unroll
     for (int k = 0; k < W; ++k) s.w[k] = __ldcs(src + k);
     int inv = M::first_violated_invariant(s);
-    if (inv >= 0) record_violation(p.ctr, p.viol_ring, s, p.parent[i & p.store_mask], fingerprint(s), (uint64_t)inv);
+    if (inv >= 0) record_violation(p.ctr, p.viol_ring, s, p.parent[i & p.store_mask], state_fp(s), (uint64_t)inv);
   }
 }
 

@@ -22,7 +22,8 @@ TLC's operational rules (SURVEY.md App. D, from the published TLC design):
   operator definitions and LET in place; everything else is a plain boolean;
 * ``states generated`` = #init + every successor produced (duplicates and self-loops count);
 * a successor violating a CONSTRAINT is counted as generated and invariant-checked but is
-  neither stored nor explored;
+  neither stored nor explored; so is an initial state violating one (``out_of_model`` counts both,
+  every generation of such a state);
 * depth = number of BFS levels, Init = level 1;
 * ``=`` between incomparable kinds (int vs record, string vs int) is an error, except that a
   model value is simply unequal to anything else.
@@ -923,7 +924,7 @@ def run_bfs(module: str, search_dirs: list[str], cfg_text: str, max_states: int 
 
     res = {
         "module": module, "distinct": 0, "generated": 0, "depth": 0, "levels": [],
-        "deadlocks": 0, "violation": None, "complete": True,
+        "deadlocks": 0, "out_of_model": 0, "violation": None, "complete": True,
         "first_violation_level": {inv: None for inv in cfg.invariants},
         "violating_states": {inv: 0 for inv in cfg.invariants},
     }
@@ -949,6 +950,7 @@ def run_bfs(module: str, search_dirs: list[str], cfg_text: str, max_states: int 
     for st in inits:
         kk = key(st)
         if not in_model(st):
+            res["out_of_model"] += 1
             check_invariants(st, 1, None)
             continue
         if kk in seen:
@@ -977,6 +979,7 @@ def run_bfs(module: str, search_dirs: list[str], cfg_text: str, max_states: int 
             for s1 in succs:
                 kk = key(s1)
                 if not in_model(s1):
+                    res["out_of_model"] += 1
                     if check_invariants(s1, level + 1, pk):
                         stop = True
                         break

@@ -1,12 +1,13 @@
 """Generates tests/golden/goldens.json -- run after `make -C oracle` (needs oracle/_ref/spec), commit the output.
 
-For every model of models/MODELS.json:
+For every registered model (models/MODELS.json and the test-only tests/specs/MODELS.json):
   * Oracle B (oracle/kspec_oracle.c, hand-written C restatement) runs the full BFS;
   * if the entry is marked "oracle_a", Oracle A (oracle/tla_interp.py, direct interpreter of the
     unchanged .tla text) runs it too, and both must agree on distinct / generated / depth /
     per-level widths / deadlocks / per-invariant first-violation level;  Oracle A also provides a
     digest of the set of reachable states (canonical TLC-style text), which the lowered model must
-    reproduce state for state;
+    reproduce state for state, and the number of states a CONSTRAINT discards (out_of_model: initial
+    states and every generation of a successor);
   * analytic closed forms (IdSequence, FiniteReplicatedLog) are asserted where they exist.
 The reference ships no goldens of its own (parity unpinned, see oracle/tla_interp.py).
 """
@@ -46,8 +47,8 @@ def closed_form(module, cfg):
 
 
 def main():
-    with open(os.path.join(ROOT, "models", "MODELS.json")) as f:
-        reg = json.load(f)
+    from kafka_specification_b200.build import registry
+    reg = registry()
     only = sys.argv[1:]
     out_path = os.path.join(HERE, "goldens.json")
     out = json.load(open(out_path)) if os.path.exists(out_path) else {}
@@ -87,6 +88,7 @@ def main():
             for inv, lvl in b["first_violation_level"].items():
                 assert a["first_violation_level"].get(inv) == lvl, (name, inv, a["first_violation_level"], lvl)
             g["first_violation_level"] = a["first_violation_level"]     # includes TypeOk
+            g["out_of_model"] = a["out_of_model"]
             if not spec.get("symmetry"):       # under SYMMETRY the choice of orbit representatives is free
                 g["state_digest"] = state_digest(a["states"])
             g["sources"].append("oracle_a")

@@ -292,13 +292,12 @@ struct Store {
 //   e = 0   stored level-1 states that violate an invariant, in-model or not (the initial states go through the insert)
 //   e >= 1  deadlocks of level e (when deadlocks are checked), stored level-(e+1) states that violate an invariant,
 //           and the out-of-model successors of level e that violate one (every generation of one, not deduplicated)
-// Row: W words, parent word, invariant (~0 = deadlock), 1 if the engine fingerprints the canonical state (the
-// out-of-model rows: the insert's identity) else 0 (k_invariants and deadlocks fingerprint the stored state).
+// Row: W words, parent word, invariant (~0 = deadlock).  The engine fingerprints every row by its canonical state.
 struct ViolationSink {
   std::vector<uint64_t>* rows;   // the rows of the first level end that has any (so far)
   uint64_t* counts;              // [n_expanded + 1] violators per level end
   uint64_t first = ~0ull;
-  void add(uint64_t e, const State& s, uint64_t meta, uint64_t inv, uint64_t canonical) {
+  void add(uint64_t e, const State& s, uint64_t meta, uint64_t inv) {
     counts[e]++;
     if (e > first) return;
     if (e < first) {
@@ -308,7 +307,6 @@ struct ViolationSink {
     for (int k = 0; k < W; ++k) rows->push_back(s.w[k]);
     rows->push_back(meta);
     rows->push_back(inv);
-    rows->push_back(canonical);
   }
 };
 std::vector<uint64_t> g_viol_rows;
@@ -346,7 +344,7 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
       totals[2]++;
       if (M::NUM_INVARIANTS > 0) {
         const int inv = M::first_violated_invariant(s);
-        if (inv >= 0) V.add(0, s, NO_PARENT, (uint64_t)inv, 1);
+        if (inv >= 0) V.add(0, s, NO_PARENT, (uint64_t)inv);
       }
       continue;
     }
@@ -425,7 +423,7 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
     // invariants of the stored states: checked by k_invariants at the end of the level that added them
     if (M::NUM_INVARIANTS > 0 && L - 1 <= n_expanded) {
       const int inv = M::first_violated_invariant(s);
-      if (inv >= 0) V.add(L - 1, s, parents[i], (uint64_t)inv, 0);
+      if (inv >= 0) V.add(L - 1, s, parents[i], (uint64_t)inv);
     }
     if (L > n_expanded) continue;
     successors(s, true, sink, site_gen);
@@ -436,7 +434,7 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
     totals[0] += sink.out.size();
     if (sink.out.empty()) {
       totals[1]++;
-      if (check_deadlock) V.add(L, s, parents[i], ~0ull, 0);
+      if (check_deadlock) V.add(L, s, parents[i], ~0ull);
     }
     for (size_t k = 0; k < sink.out.size(); ++k) {
       const State& t = sink.out[k];
@@ -445,7 +443,7 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
         totals[2]++;
         if (M::NUM_INVARIANTS > 0) {
           const int inv = M::first_violated_invariant(t);
-          if (inv >= 0) V.add(L, t, S.parent_ref(i) | ((uint64_t)sink.act[k] << 56), (uint64_t)inv, 1);
+          if (inv >= 0) V.add(L, t, S.parent_ref(i) | ((uint64_t)sink.act[k] << 56), (uint64_t)inv);
         }
         continue;
       }
@@ -463,7 +461,7 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
 
 // the violator rows of the first level end with any, from the last audit_store call; returns the number of rows
 uint64_t audit_violator_rows(uint64_t* out, uint64_t cap) {
-  const uint64_t row = W + 3, n = g_viol_rows.size() / row;
+  const uint64_t row = W + 2, n = g_viol_rows.size() / row;
   memcpy(out, g_viol_rows.data(), std::min(n, cap) * row * 8);
   return n;
 }
@@ -557,7 +555,7 @@ void hs_insert(void* h, const uint64_t* rows, uint64_t n) {
     }
     if (is_new || !inmodel) {
       const int inv = M::first_violated_invariant(s);
-      const uint64_t fp = fingerprint(s);
+      const uint64_t fp = fingerprint(canon(s));   // the engine's pick: by set identity, the orbit's under SYMMETRY
       if (inv >= 0 && (r->viol_inv < 0 || r->viol_level == r->level + 1) && fp < r->viol_fp) {
         if (r->viol_inv < 0) r->viol_level = r->level + 1;
         r->viol_inv = inv;

@@ -29,7 +29,8 @@ class LabelledInterp(tla_interp.Interp):
         super().__init__(root, cfg)
         self.generated: Counter = Counter()
 
-    def next_states(self, next_expr, st: dict) -> list[dict]:
+    def labelled_successors(self, next_expr, st: dict) -> list[tuple[dict, str]]:
+        """The successors of `st` under Next, each with the name of the action that produced it."""
         start = (next_expr, self.root, None, {})
         if next_expr[0] == "id":
             # the body of Next: Next itself is not an action (the lowering starts at the same place)
@@ -38,6 +39,10 @@ class LabelledInterp(tla_interp.Interp):
                 start = (r.defn.body, r.ctx, r.defn.module, {})
         out: list[tuple[dict, str]] = []
         self._next_l([start], st, {}, out, None)
+        return out
+
+    def next_states(self, next_expr, st: dict) -> list[dict]:
+        out = self.labelled_successors(next_expr, st)
         for _, label in out:
             self.generated[label] += 1
         return [s1 for s1, _ in out]

@@ -178,7 +178,7 @@ class AuditLib(HostModel):
         if rc != 0:
             raise AuditError(f"{msg.value.decode()}  [{self.name}]")
         n_rows = int(self.lib.audit_violator_rows(None, 0))
-        rows = np.zeros((n_rows, self.words + 3), dtype=np.uint64)
+        rows = np.zeros((n_rows, self.words + 2), dtype=np.uint64)
         if n_rows:
             self.lib.audit_violator_rows(rows.ctypes.data, n_rows)
         return {"generated": int(totals[0]), "deadlocks": int(totals[1]), "out_of_model": int(totals[2]),
@@ -190,23 +190,23 @@ class AuditLib(HostModel):
 # ------------------------------------------------------------------------------------------------ the audit proper
 def expected_violation(a: AuditLib, found: dict) -> dict | None:
     """build_trace's pick among the violators of the first level end that has any: deadlocks first, then the smallest
-    fingerprint, then the smallest parent word.  The engine fingerprints out-of-model violators by their canonical
-    state (the insert's identity) and the others by the stored state itself."""
+    fingerprint, then the smallest parent word.  The engine fingerprints every violator, stored or discarded by a
+    CONSTRAINT, by its canonical state (its set identity), so under SYMMETRY the pick does not depend on which member
+    of an orbit was stored."""
     counts = found["violators_per_level_end"]
     ends = [e for e, c in enumerate(counts) if c]
     if not ends:
         return None
     rows = found["violators"]
     w = a.words
-    fps = a.fingerprints(rows[:, :w], rows[:, w + 2] == 1)
+    fps = a.fingerprints(rows[:, :w], True)
     dead = rows[:, w + 1] == np.uint64(M64)
     order = np.lexsort((rows[:, w], fps, ~dead))          # last key first: deadlocks, fingerprint, parent word
     best = int(order[0])
     return {"level_end": ends[0], "count": int(counts[ends[0]]), "rows": rows, "fps": fps, "dead": dead,
             "kind": "deadlock" if dead[best] else "invariant", "invariant": None if dead[best] else int(rows[best, w + 1]),
             "level": ends[0] if dead[best] else ends[0] + 1, "fingerprint": int(fps[best]),
-            "words": [int(x) for x in rows[best, :w]], "parent_word": int(rows[best, w]),
-            "canonical": bool(rows[best, w + 2] == 1)}
+            "words": [int(x) for x in rows[best, :w]], "parent_word": int(rows[best, w])}
 
 
 def compare(a: AuditLib, found: dict, *, stats: dict, coverage: dict | None, parents: np.ndarray,
@@ -259,7 +259,7 @@ def compare(a: AuditLib, found: dict, *, stats: dict, coverage: dict | None, par
         if (list(record[0]), record[1]) != (want["words"], want["parent_word"]):
             raise AuditError(f"counterexample: kmc_violation_record {record} is not the picked violator "
                              f"{(want['words'], want['parent_word'])}")
-        fp = int(a.fingerprints(np.asarray([record[0]], dtype=np.uint64), want["canonical"])[0])
+        fp = int(a.fingerprints(np.asarray([record[0]], dtype=np.uint64), True)[0])
         if fp != violation["fingerprint"]:
             raise AuditError(f"counterexample: the record's words hash to {fp:#x}, the run reports "
                              f"{violation['fingerprint']:#x}")
