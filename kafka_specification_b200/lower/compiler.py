@@ -58,8 +58,34 @@ class Closure:
         self.defn, self.ctx, self.fm, self.env = defn, ctx, fm, env
 
 
+class Block:
+    """A block of emitted C: its head (``if (...)``, or empty for a bare block), the condition the head tests and
+    its children, which are statements (strings) and blocks.  A block with a ``label`` is a core: the bare block
+    emit_successor() opens, which builds one successor and emits it with that action label (-1: the core only
+    reports a layout trap), with no further branching on the state."""
+    __slots__ = ("head", "cond", "label", "children")
+
+    def __init__(self, head: str = "", cond: str | None = None, label: int | None = None, children=None):
+        self.head, self.cond, self.label = head, cond, label
+        self.children: list = [] if children is None else children
+
+
+def render(nodes: list, depth: int) -> list[str]:
+    """The C text of a tree: one statement, block head or closing brace per line, two spaces per level."""
+    out = []
+    for n in nodes:
+        pad = "  " * depth
+        if isinstance(n, Block):
+            out.append(pad + (n.head + " {" if n.head else "{"))
+            out.extend(render(n.children, depth + 1))
+            out.append(pad + "}")
+        else:
+            out.append(pad + n)
+    return out
+
+
 class CG:
-    """Structured C emitter with block-scoped temporaries.
+    """Structured C emitter with block-scoped temporaries; it builds the function body as a tree of Blocks.
 
     ``root`` is the block id of the function body; a fresh CG continuing the same function
     prologue (``fork``) keeps the root id and the prologue's CSE table, so that values computed in
@@ -67,11 +93,10 @@ class CG:
     _ids = itertools.count(1)
 
     def __init__(self, root: int | None = None, cse: dict | None = None, next_tmp: int = 0):
-        self.lines: list[str] = []
-        self.depth = 1
+        self.body = Block()
+        self.stack = [self.body]              # the open blocks, outermost first
         self.root = next(CG._ids) if root is None else root
-        self.blocks = [self.root]
-        self.conds: list[str | None] = [None]
+        self.blocks = [self.root]             # their ids (the scopes of CSE hits)
         self.next_tmp = next_tmp
         self.cse: dict[tuple[str, str], tuple[str, int]] = dict(cse or {})
 
@@ -79,22 +104,21 @@ class CG:
         return CG(self.root, {k: v for k, v in self.cse.items() if v[1] == self.root}, self.next_tmp)
 
     def pristine(self) -> bool:
-        return not self.lines and self.depth == 1
+        return not self.body.children and len(self.stack) == 1
 
     def emit(self, s: str):
-        self.lines.append("  " * self.depth + s)
+        self.stack[-1].children.append(s)
 
-    def open(self, head: str = "", cond: str | None = None):
-        self.emit(head + " {" if head else "{")
-        self.depth += 1
+    def open(self, head: str = "", cond: str | None = None, label: int | None = None) -> Block:
+        b = Block(head, cond, label)
+        self.stack[-1].children.append(b)
+        self.stack.append(b)
         self.blocks.append(next(CG._ids))
-        self.conds.append(cond)
+        return b
 
     def close(self):
-        self.depth -= 1
+        self.stack.pop()
         self.blocks.pop()
-        self.conds.pop()
-        self.emit("}")
 
     def tmp(self, ctype: str, expr: str) -> str:
         key = (ctype, expr)
@@ -108,14 +132,14 @@ class CG:
         return name
 
     def mark(self):
-        if self.depth != len(self.blocks):
-            raise LowerError("internal: unbalanced blocks")
-        return (len(self.lines), self.next_tmp, dict(self.cse))
+        return (self.stack[-1], len(self.stack[-1].children), self.next_tmp, dict(self.cse))
 
     def rollback(self, m):
-        del self.lines[m[0]:]
-        self.next_tmp = m[1]
-        self.cse = m[2]
+        if self.stack[-1] is not m[0]:
+            raise LowerError("internal: unbalanced blocks")
+        del m[0].children[m[1]:]
+        self.next_tmp = m[2]
+        self.cse = m[3]
 
 
 class Lowerer:
@@ -141,9 +165,8 @@ class Lowerer:
         self.layout: L.Layout | None = None
         self.actions: list[dict] = []         # {"name", "module", "line", "col", ...}
         self.emit_sites = 0
-        self.units: list[tuple[list[str], int]] = []   # (lines, emit sites) of independently compilable pieces
+        self.units: list[list] = []                    # trees of the independently compilable pieces
         self.unit_id = 0
-        self._unit_emit_mark = 0
         self.prologue: list[str] = []
         self.enc_cache: dict[int, tuple] = {}          # id(sval) -> (type sig, sval, code expr) for values decoded from a code
         self.mux_origin: dict[int, tuple] = {}         # id(sval) -> (sval, cond, a, b) for composite selects
@@ -1532,7 +1555,7 @@ class Lowerer:
         if cond is True:
             body()
             return
-        if cond.s in self.cg.conds:
+        if any(b.cond == cond.s for b in self.cg.stack):
             body()
             return
         self.cg.open(f"if ({cond.s})", cond.s)
@@ -1541,11 +1564,10 @@ class Lowerer:
 
     def end_unit(self):
         """Close the current independently-compilable piece of expand() and start a new one."""
-        if self.cg.depth != 1:
+        if len(self.cg.stack) != 1:
             raise LowerError("internal: end_unit inside an open block")
-        if self.cg.lines:
-            self.units.append((self.cg.lines, self.emit_sites - self._unit_emit_mark))
-        self._unit_emit_mark = self.emit_sites
+        if self.cg.body.children:
+            self.units.append(self.cg.body.children)
         self.unit_id += 1
         self.cg = self._unit_base.fork()
 
@@ -1569,7 +1591,7 @@ class Lowerer:
         if label is None:
             label = self.action_id(Def("Next", [], ("id", "Next"), False, self.root.module_name))
         lay = self.layout
-        self.cg.open()
+        core = self.cg.open(label=label)
         self.traps = []
         out: dict[int, str] = {}
         for v in self.variables:
@@ -1586,6 +1608,7 @@ class Lowerer:
                 continue
             by_word.setdefault(a.word, []).append((a, code))
         if ok is False:
+            core.label = -1
             self.cg.emit("sink.fail(KMC_FAIL_LAYOUT);")
             self.cg.close()
             return
@@ -1699,17 +1722,17 @@ class Lowerer:
         self.mux_origin = {}
         self.unit_id = -2                      # values forced while reading belong to the prologue
         self.cur = {v: self.read_ty(self.layout.var_types[v]) for v in self.variables}
-        self.prologue = self.cg.lines
-        self.cg.lines = []
+        self.prologue = render(self.cg.body.children, 1)
+        self.cg.body.children = []
         self._unit_base = self.cg
         self.units = []
         self.unit_id = 0
-        self._unit_emit_mark = self.emit_sites
         self.cg = self._unit_base.fork()
 
     def unpack_lines(self) -> list[str]:
         out = []
         for a in self.layout.atoms:
             sh = f" >> {a.shift}" if a.shift else ""
-            out.append(f"  const unsigned a{a.index} = (unsigned)((s.w[{a.word}]{sh}) & 0x{a.mask:x}ull);  // {a.path}")
+            out.append(f"  [[maybe_unused]] const unsigned a{a.index} = (unsigned)((s.w[{a.word}]{sh}) & 0x{a.mask:x}ull);"
+                       f"  // {a.path}")
         return out

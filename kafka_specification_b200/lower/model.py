@@ -11,7 +11,6 @@ from __future__ import annotations
 import copy
 import hashlib
 import json
-import re
 from dataclasses import dataclass, field
 
 from ..frontend.cfg import Config, ModelValue, parse_cfg
@@ -19,7 +18,7 @@ from ..frontend.modules import ModuleContext, load_root
 from ..frontend.tla_parser import parse_expression_text
 from ..frontend.values import FnVal, fmt, sort_key
 from . import layout as L
-from .compiler import Closure, Lowerer, Marker, Thunk
+from .compiler import Block, Closure, Lowerer, Marker, Thunk, render
 from .svals import LowerError, SLazy, is_atom_const, is_const, is_int_const
 
 LOWERING_VERSION = 3
@@ -266,149 +265,93 @@ class TypeInference:
 # ---------------------------------------------------------------------------
 # guard/body decomposition of the emitted units ("items")
 # ---------------------------------------------------------------------------
-class _Node:
-    __slots__ = ("text", "cond", "children", "is_block")
-
-    def __init__(self, text, cond=None, is_block=False):
-        self.text, self.cond, self.is_block, self.children = text, cond, is_block, []
-
-
-def _parse_unit(lines: list[str]) -> list[_Node]:
-    """Parses the emitter's own output (one statement / block head / '}' per line) into a tree."""
-    root = _Node("", is_block=True)
-    stack = [root]
-    for raw in lines:
-        t = raw.strip()
-        if t == "}":
-            stack.pop()
-        elif t.endswith("{"):
-            cond = t[len("if ("):-len(") {")] if t.startswith("if (") else None
-            n = _Node(t, cond, True)
-            stack[-1].children.append(n)
-            stack.append(n)
-        else:
-            stack[-1].children.append(_Node(t))
-    if len(stack) != 1:
-        raise LowerError("internal: unbalanced unit")
-    return root.children
-
-
-def _prune(nodes: list[_Node]) -> list[_Node]:
+def _prune(nodes: list) -> list:
+    """A copy of the tree without its empty blocks (e.g. statically dead disjuncts)."""
     out = []
     for n in nodes:
-        if n.is_block:
-            n.children = _prune(n.children)
-            if not n.children:
-                continue            # empty block (e.g. a statically dead disjunct)
+        if isinstance(n, Block):
+            kids = _prune(n.children)
+            if not kids:
+                continue
+            n = Block(n.head, n.cond, n.label, kids)
         out.append(n)
     return out
 
 
-def _render(nodes: list[_Node], depth: int) -> list[str]:
-    out = []
-    for n in nodes:
-        if n.is_block:
-            out.append("  " * depth + n.text)
-            out.extend(_render(n.children, depth + 1))
-            out.append("  " * depth + "}")
-        else:
-            out.append("  " * depth + n.text)
-    return out
-
-
-def _split_unit(lines: list[str], max_blocks: int) -> list[list[str]]:
-    """Cuts a unit with many top-level blocks (e.g. an enumeration over an 80-element bitmap set) into
+def _split_unit(nodes: list, max_blocks: int) -> list[list]:
+    """Cuts a pruned unit with many top-level blocks (e.g. an enumeration over an 80-element bitmap set) into
     sub-units of at most ``max_blocks`` blocks; the unit's root-level temporaries are pure and are
     replicated in every sub-unit."""
-    nodes = _prune(_parse_unit(lines))
-    temps = [n for n in nodes if not n.is_block and not n.text.startswith("else ")]
-    chunks: list[list[_Node]] = [[]]
-    count = 0
-    for n in nodes:
-        if n.is_block:
-            if count == max_blocks:
-                chunks.append([])
-                count = 0
-            chunks[-1].append(n)
-            count += 1
-        elif n.text.startswith("else "):
-            chunks[-1].append(n)
-    return [[l[2:] if l.startswith("  ") else l for l in _render(temps + c, 1)] for c in chunks if c]
+    temps = [n for n in nodes if not isinstance(n, Block)]
+    blocks = [n for n in nodes if isinstance(n, Block)]
+    return [temps + blocks[i:i + max_blocks] for i in range(0, len(blocks), max_blocks)]
 
 
-def _is_core(n: _Node) -> bool:
-    """A core is the bare block emit_successor() opens: it packs and emits exactly one successor (or
-    reports a layout trap) and contains no further branching on the state."""
-    if not n.is_block or n.cond is not None or n.text != "{":
-        return False
-    for k in n.children:
-        if not k.is_block and (k.text.startswith("State n = s;") or k.text.startswith("sink.fail(")):
-            return True
-        if k.is_block and any((not c.is_block) and c.text.startswith("State n = s;") for c in k.children):
-            return True
-    return False
+def _site_core(n: Block) -> Block | None:
+    """The core of the emit site that block ``n`` is, or None.  A site is a core, or else a bare block (one disjunct
+    of an `\\/`) holding only temporaries and one core that emits without a layout check: such a block is a site
+    as a whole and its body keeps the block.  The kip101 and kip279 models have such blocks, and their generated
+    headers (hence their device code) are cut this way."""
+    if n.label is not None:
+        return n
+    blocks = [k for k in n.children if isinstance(k, Block)]
+    if n.head or len(blocks) != 1:
+        return None
+    core = blocks[0]
+    unchecked = core.label is not None and core.label >= 0 and not any(isinstance(k, Block) for k in core.children)
+    return core if unchecked else None
 
 
-def _unit_sites(lines: list[str]):
-    """Splits one unit into emit sites.  Returns (guard_tree, sites):
+def _unit_sites(nodes: list):
+    """Splits one pruned unit into emit sites, one per core.  Returns (guard_tree, sites):
 
-    * ``guard_tree`` is the unit's own code with every core replaced by a marker node ``@site k`` (k = index
-      of the site inside the unit); rendered by ``_render_guard`` it evaluates, for one state, the COMPLETE
-      path condition of every site (all the `if`s between the unit root and the core), sharing the common
-      prefixes exactly as expand() does;
-    * ``sites[k]`` = body lines of site k: the (pure, hence safely speculated) temporaries of the blocks on
-      its path, flattened, followed by the core.  The body does not re-check the path condition: it is run
-      only for (state, site) pairs whose mask bit is set.
+    * ``guard_tree`` is the unit's own code with every site's block replaced by its site index k (within the
+      unit); rendered by ``_render_guard`` it evaluates, for one state, the COMPLETE path condition of every site
+      (all the `if`s between the unit root and the site), sharing the common prefixes exactly as expand() does;
+    * ``sites[k]`` = (action label of its core, body lines) of site k.  The body is the (pure, hence safely
+      speculated) temporaries of the blocks on its path, flattened, followed by the site's block.  It does not
+      re-check the path condition: it is run only for (state, site) pairs whose mask bit is set.
     """
-    nodes = _prune(_parse_unit(lines))
-    sites: list[list[str]] = []
+    sites: list[tuple[int, list[str]]] = []
 
-    def walk(ns: list[_Node], path_temps: list[_Node]) -> list[_Node]:
-        out: list[_Node] = []
-        temps_here: list[_Node] = []
+    def walk(ns: list, path_temps: list[str]) -> list:
+        out: list = []
+        temps_here: list[str] = []
         for n in ns:
-            if not n.is_block:
-                if not n.text.startswith("const "):
-                    raise LowerError(f"internal: statement outside a core: {n.text}")
+            if not isinstance(n, Block):
                 temps_here.append(n)
                 out.append(n)
-                continue
-            if _is_core(n):
-                out.append(_Node(f"@site {len(sites)}"))
-                sites.append(_render(path_temps + temps_here, 1) + _render([n], 1))
-                continue
-            blk = _Node(n.text, n.cond, True)
-            blk.children = walk(n.children, path_temps + temps_here)
-            out.append(blk)
+            elif (core := _site_core(n)) is not None:
+                out.append(len(sites))
+                sites.append((core.label, render(path_temps + temps_here, 1) + render([n], 1)))
+            else:
+                out.append(Block(n.head, n.cond, None, walk(n.children, path_temps + temps_here)))
         return out
 
     return walk(nodes, []), sites
 
 
-def _render_guard(tree: list[_Node], lo: int, hi: int, bit0: int) -> list[str]:
+def _render_guard(tree: list, lo: int, hi: int, bit0: int) -> list[str]:
     """Guard code of the sites lo <= k < hi of one unit: site k sets mask bit (bit0 + k - lo).  Blocks without a
     site in the window are dropped; temporaries stay (the C++ compiler removes the unused ones)."""
     def prune(ns):
         out, live = [], False
         for n in ns:
-            if n.is_block:
+            if isinstance(n, Block):
                 sub, sub_live = prune(n.children)
                 if sub_live:
-                    blk = _Node(n.text, n.cond, True)
-                    blk.children = sub
-                    out.append(blk)
+                    out.append(Block(n.head, n.cond, None, sub))
                     live = True
-            elif n.text.startswith("@site "):
-                k = int(n.text[6:])
-                if lo <= k < hi:
-                    out.append(_Node(f"m |= 1ull << {bit0 + k - lo};"))
+            elif isinstance(n, int):
+                if lo <= n < hi:
+                    out.append(f"m |= 1ull << {bit0 + n - lo};")
                     live = True
             else:
                 out.append(n)
         return out, live
 
     nodes, live = prune(tree)
-    return _render(nodes, 1) if live else []
+    return render(nodes, 2) if live else []
 
 
 # ---------------------------------------------------------------------------
@@ -468,18 +411,6 @@ def _init_states(lw: Lowerer, init_expr) -> list[dict]:
 
     rec([(init_expr, lw.root, None, {})], {})
     return out
-
-
-_EMIT_LABEL = re.compile(r"sink\.emit\(n, (\d+)\);")
-
-
-def _site_action(body: list[str]) -> int:
-    """The action of an emit site: the label of the one sink.emit in its core (-1 for a core that only reports a
-    layout trap; reaching it fails the run)."""
-    labels = {int(x) for line in body for x in _EMIT_LABEL.findall(line)}
-    if len(labels) > 1:
-        raise LowerError("internal: an emit site carries more than one action label")
-    return labels.pop() if labels else -1
 
 
 def _init_info(lw: Lowerer, init_e, module: str) -> dict:
@@ -644,17 +575,22 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     # One-phase form: consecutive units packed into groups of bounded size, one function each; expand() calls them
     # in order.  The host tests, the CPU baseline and the host-side shard stand-ins run it; the CUDA build skips
     # this section of the header (-DKMC_NO_ONE_PHASE) to keep nvcc time down.
+    # A unit's one-phase text keeps its empty blocks; a split unit's is its pruned sub-units, one level shallower.
+    # The body digest, which checkpoints are checked against, hashes this text.
     groups: list[list[str]] = []
     cur_lines: list[str] = []
-    all_units: list[list[str]] = []
-    for lines, _ in lw.units:
-        top_blocks = sum(1 for n in _prune(_parse_unit(lines)) if n.is_block)
-        all_units.extend(_split_unit(lines, 40) if top_blocks > 40 else [lines])
-    for lines in all_units:
+    all_units: list[tuple[list, list[str]]] = []      # (pruned tree, one-phase text)
+    for nodes in lw.units:
+        pruned = _prune(nodes)
+        if sum(isinstance(n, Block) for n in pruned) > 40:
+            all_units.extend((sub, render(sub, 1)) for sub in _split_unit(pruned, 40))
+        else:
+            all_units.append((pruned, render(nodes, 2)))
+    for _, lines in all_units:
         if cur_lines and len(cur_lines) + len(lines) > GROUP_LINES:
             groups.append(cur_lines)
             cur_lines = []
-        cur_lines = cur_lines + ["  {"] + ["  " + l for l in lines] + ["  }"]
+        cur_lines = cur_lines + ["  {"] + lines + ["  }"]
     if cur_lines or not groups:
         groups.append(cur_lines)
     expand_lines = [l for g in groups for l in g]
@@ -662,8 +598,9 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     # condition, straight-line body).  A site group = a run of consecutive sites (<= 64: one mask word; bounded
     # guard code so that the guard phase of a group stays in the instruction cache); a unit with more sites than
     # fit is covered by several windows of the same guard tree.
-    unit_trees = [_unit_sites(lines) for lines in all_units]
+    unit_trees = [_unit_sites(nodes) for nodes, _ in all_units]
     site_bodies: list[list[str]] = []
+    site_action: list[int] = []
     site_groups: list[dict] = []            # {"begin": first site, "count": n, "guard": lines}
     cur = {"begin": 0, "count": 0, "guard": []}
     for tree, sites in unit_trees:
@@ -676,18 +613,17 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
                 continue
             n = min(room, len(sites) - k)
             g = _render_guard(tree, k, k + n, cur["count"])
-            cur["guard"] += ["  {"] + ["  " + l for l in g] + ["  }"]
+            cur["guard"] += ["  {"] + g + ["  }"]
             cur["count"] += n
             k += n
-        site_bodies.extend(sites)
+        site_action.extend(label for label, _ in sites)
+        site_bodies.extend(body for _, body in sites)
     if cur["count"] or not site_groups:
         site_groups.append(cur)
     max_fanout = lw.emit_sites
 
     # invariants
     lw.begin_function()
-    inv_prologue = list(lw.prologue)
-    inv_lines_start = len(lw.cg.lines)
     for i, inv in enumerate(cfg.invariants):
         idf, ictx = lw.named_def(inv)
         c = lw.ev_bool(idf.body, ictx, idf.module, {})
@@ -695,7 +631,7 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
             lw.cg.emit(f"return {i};")
         elif c is not True:
             lw.cg.emit(f"if (!({c.s})) return {i};")
-    inv_lines = inv_prologue + lw.cg.lines[inv_lines_start:]
+    inv_lines = lw.prologue + render(lw.cg.body.children, 1)
 
     # constraints
     lw.begin_function()
@@ -704,8 +640,7 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
         cdf, cctx = lw.named_def(con)
         conds.append(lw.ev_bool(cdf.body, cctx, cdf.module, {}))
     c_all = lw.b_and(conds)
-    con_lines = list(lw.prologue) + list(lw.cg.lines)
-    con_lines.append(f"  return {lw.bstr(c_all)};")
+    con_lines = lw.prologue + render(lw.cg.body.children, 1) + [f"  return {lw.bstr(c_all)};"]
 
     # SYMMETRY: canonicalize(s) = lexicographically smallest packed image of s under the symmetry group
     sym_lines: list[str] = []
@@ -728,7 +663,7 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
                 lw.cg.emit(f"c.w[{w}] = {e};")
             lw.cg.emit("if (state_less(c, best)) best = c;")
             lw.cg.close()
-        sym_lines = list(lw.prologue) + list(lw.cg.lines)
+        sym_lines = lw.prologue + render(lw.cg.body.children, 1)
 
     name = name or module
     if len(lw.actions) > 255:
@@ -769,7 +704,6 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     parts.append("#endif  // KMC_NO_ONE_PHASE")
     n_sites = len(site_bodies)
     parts.append(f"static constexpr int NUM_SITES = {n_sites};")
-    site_action = [_site_action(body) for body in site_bodies]
     parts.append("/* action of every emit site (index into the model's actions; -1: the site only reports a layout trap) */")
     parts.append("static constexpr int SITE_ACTION[NUM_SITES > 0 ? NUM_SITES : 1] = {" +
                  (", ".join(str(a) for a in site_action) if site_action else "-1") + "};")
@@ -837,7 +771,6 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     parts.append("}")
     parts.append("}  // namespace kmc_model")
     header = "\n".join(parts) + "\n"
-    header = header.replace("  const unsigned a", "  [[maybe_unused]] const unsigned a")
 
     return LoweredModel(
         name=name, module=module, header=header, layout=lay.describe(), words=lay.words,
