@@ -17,6 +17,7 @@
  *   kmc_stats           ModelChecker.reportSuccess / printSummary ("N states generated,
  *                       M distinct states found, Q states left on queue", depth)
  *   kmc_violation       ModelChecker.doNext's invariant/deadlock failure report
+ *   kmc_invariant_*     the same per invariant under -continue (first level, violators, counterexample)
  *   kmc_coverage        ModelChecker's coverage report (TLC -coverage: "distinct:generated" per action, at the
  *                       action level of TLC >= 1.7), from counters the kernels keep on every run
  *   kmc_trace_*         tlc2.tool.TLCTrace.getTrace / printTrace (error trace by parent links)
@@ -92,6 +93,16 @@ typedef struct {
                                its orbit (the canonical form), whichever member was reached  */
 } kmc_violation_t;
 
+/* One violated invariant of a "continue" run (kmc_invariant_reports). */
+typedef struct {
+  int32_t invariant;              /* index into the cfg's INVARIANT list                              */
+  uint64_t level;                 /* first BFS level with a checked state that violates it (Init = 1) */
+  uint64_t violators_first_level; /* checked states of that level that violate it                     */
+  uint64_t violators;             /* ... over the whole run                                           */
+  uint64_t trace_len;             /* states in its counterexample (= level)                           */
+  uint64_t fingerprint;           /* set-identity fingerprint of the counterexample's last state      */
+} kmc_invariant_report_t;
+
 typedef struct {
   int32_t words;            /* 64-bit words per packed state                              */
   int32_t state_bits;
@@ -146,6 +157,18 @@ int kmc_coverage(const kmc_ctx* ctx, uint64_t* action_generated, uint64_t* actio
 int kmc_violation(const kmc_ctx* ctx, kmc_violation_t* out);
 /* i-th state of the error trace (0 = an initial state); buf receives `words` uint64_t.    */
 int kmc_trace_state(const kmc_ctx* ctx, uint32_t i, uint64_t* buf, size_t cap_words, uint32_t* action_id);
+/* Every violated invariant of the last run with "continue": true, ordered by (level, invariant); invariants never
+ * violated are absent, and deadlocks stay in kmc_violation.  "Checked" states are the stored states and the successors
+ * a CONSTRAINT discards (each time one is generated).  Each report's counterexample is, among the violators of its
+ * first level, the one kmc_violation's rule picks (smallest fingerprint, then smallest parent word); so when
+ * kmc_violation reports an invariant, it is that invariant's entry here (as long as the level's violators fit the
+ * 2^16-row ring: beyond that neither pick is deterministic).  Up to cap entries are written, *n receives the full
+ * count.  *complete = 0 after -recover: the report then covers only the levels searched since.  KMC_E_BADARG on a
+ * model with more than 64 invariants; KMC_E_STATE on one rank of a multi-process (kmc_shard_*, world > 1) driver.  */
+int kmc_invariant_reports(const kmc_ctx* ctx, kmc_invariant_report_t* out, size_t cap, size_t* n, int32_t* complete);
+/* i-th state of the counterexample of invariant `invariant` (0 = an initial state), as kmc_trace_state.           */
+int kmc_invariant_trace_state(const kmc_ctx* ctx, int32_t invariant, uint32_t i, uint64_t* buf, size_t cap_words,
+                              uint32_t* action_id);
 /* copy packed states [first, first+count) of the state store to host memory               */
 int kmc_copy_states(const kmc_ctx* ctx, uint64_t first, uint64_t count, uint64_t* buf);
 /* parent words of the same range: bits 0..39 store index, 40..47 owner rank of the parent,
@@ -205,7 +228,8 @@ int kmc_shard_insert_p2p(kmc_ctx* ctx);
  *                       the same number of times per level (count = 0 on ranks without work)
  * kmc_shard_level_sync  invariants + publish this rank's level summary to all ranks + wait for all summaries; the ONE
  *                       host synchronisation of a level.  board receives world x 8 words per rank:
- *                       {level id, new states, violations, store tail, generated, fail, deadlocks, -}
+ *                       {level id, new states, violations, store tail, generated, fail, deadlocks,
+ *                        invariants first violated at this level (bit mask, "continue" runs)}
  * kmc_shard_inbox_ptr / kmc_shard_open_peers_direct: peers inside one process (one ctx per GPU, host threads):
  *                       direct device pointers + cudaDeviceEnablePeerAccess instead of CUDA IPC handles.           */
 int kmc_shard_round_p2p(kmc_ctx* ctx, uint64_t first, uint64_t count, int seed);

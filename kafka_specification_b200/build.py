@@ -7,6 +7,7 @@ Artifacts go to ``build/`` (git-ignored):
 
     build/libkspecmc.so                 the C-ABI dispatcher (include/kspecmc.h)
     build/models/<name>/model.h         the lowered switch table
+    build/models/<name>/invariants.h    violated_invariants(): the cfg's invariants as a bit mask (after model.h)
     build/models/<name>/model.json      layout / actions / invariants (for trace printing)
     build/models/<name>/libkmc_<name>.so
 
@@ -33,6 +34,7 @@ TEST_SPECS_DIR = os.path.join(ROOT, "tests", "specs")
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 SPEC_DIR = os.path.join(ROOT, "oracle", "_ref", "spec")
+INVARIANTS_HEADER = "invariants.h"
 
 
 def tla_search_dirs() -> list[str]:
@@ -89,7 +91,7 @@ def _engine_stamp() -> str:
 
 
 def lower_to_dir(module: str, cfg_path: str, name: str):
-    """Lower and write model.h / model.json; returns the LoweredModel."""
+    """Lower and write model.h / invariants.h / model.json; returns the LoweredModel."""
     import time
     from .lower.model import lower_model
     with open(cfg_path) as f:
@@ -99,11 +101,12 @@ def lower_to_dir(module: str, cfg_path: str, name: str):
     lower_seconds = time.time() - t0
     d = model_dir(name)
     os.makedirs(d, exist_ok=True)
-    hdr = os.path.join(d, "model.h")
-    old = open(hdr).read() if os.path.exists(hdr) else None
-    if old != m.header:
-        with open(hdr, "w") as f:
-            f.write(m.header)
+    for fname, text in (("model.h", m.header), (INVARIANTS_HEADER, m.invariants_header)):
+        hdr = os.path.join(d, fname)
+        old = open(hdr).read() if os.path.exists(hdr) else None
+        if old != text:
+            with open(hdr, "w") as f:
+                f.write(text)
     meta = m.meta()
     meta["cfg"] = os.path.relpath(cfg_path, ROOT)
     meta["lower_seconds"] = round(lower_seconds, 2)      # parse + lower on the build host (part of a cold start)
@@ -113,11 +116,12 @@ def lower_to_dir(module: str, cfg_path: str, name: str):
 
 
 def _nvcc_cmd(hdr: str, out_so: str) -> list[str]:
-    """nvcc of the engine with a lowered header.  The engine runs the two-phase form of the lowered Next only, so
-    -DKMC_NO_ONE_PHASE drops the one-phase form from the translation unit (it would only add nvcc time)."""
+    """nvcc of the engine with a lowered header and its invariants.h.  The engine runs the two-phase form of the lowered
+    Next only, so -DKMC_NO_ONE_PHASE drops the one-phase form from the translation unit (it would only add nvcc time)."""
     return [nvcc_path(), *NVCC_ARCH, "-lineinfo", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
-            "-diag-suppress", "177", "-DKMC_NO_ONE_PHASE",
-            f"-I{INCLUDE}", "-include", hdr, os.path.join(CSRC, "kmc_engine.cu"), "-o", out_so]
+            "-diag-suppress", "177", "-DKMC_NO_ONE_PHASE", f"-I{INCLUDE}", "-include", hdr,
+            "-include", os.path.join(os.path.dirname(hdr), INVARIANTS_HEADER), os.path.join(CSRC, "kmc_engine.cu"),
+            "-o", out_so]
 
 
 def compile_model(name: str, force: bool = False, verbose_ptxas: bool = True) -> str:
@@ -125,8 +129,11 @@ def compile_model(name: str, force: bool = False, verbose_ptxas: bool = True) ->
     hdr = os.path.join(d, "model.h")
     so = model_lib_path(name)
     stamp_file = os.path.join(d, "build.stamp")
-    with open(hdr, "rb") as f:
-        stamp = hashlib.sha256(f.read()).hexdigest()[:16] + ":" + _engine_stamp()
+    h = hashlib.sha256()
+    for p in (hdr, os.path.join(d, INVARIANTS_HEADER)):
+        with open(p, "rb") as f:
+            h.update(f.read())
+    stamp = h.hexdigest()[:16] + ":" + _engine_stamp()
     if not force and os.path.exists(so) and os.path.exists(stamp_file) and open(stamp_file).read() == stamp:
         return so
     cmd = _nvcc_cmd(hdr, so)

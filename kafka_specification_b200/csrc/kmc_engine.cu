@@ -19,7 +19,10 @@
 //                   the same over the regions the peers filled.
 //   k_invariants (K3) the cfg's INVARIANTs on the new states of a level (compacted => every lane busy).
 //                   Violating states (rare, terminal) go to a small ring; the host reports the one with
-//                   the smallest fingerprint, so the counterexample is deterministic.
+//                   the smallest fingerprint, so the counterexample is deterministic.  Under "continue",
+//                   k_invariant_report then passes a level's violators through record_invariants: violators
+//                   per invariant, and a second ring that holds the violators of invariants not reported
+//                   yet, so that every invariant gets its own first level and counterexample.
 //
 // DESIGN.md sections 3-4 give the layout, the kernels and their measurements.
 //
@@ -169,6 +172,14 @@ struct DevCounters {
   // coverage (TLC -coverage), kept over all levels of a run:
   unsigned long long site_generated[M::NUM_SITES > 0 ? M::NUM_SITES : 1];   // successors per emit site (K1's A1 totals)
   unsigned long long action_distinct[M::NUM_ACTIONS];   // new states per action (K2, from the winners' parent words)
+  // per-invariant report (kmc_invariant_reports), kept by record_invariants when inv_on is set ("continue"):
+  unsigned long long inv_on;
+  unsigned long long inv_pending;        // invariants not reported yet: only their violators take rows (host-written)
+  unsigned long long inv_new;            // pending invariants violated since the last level end
+  unsigned long long inv_rows;           // rows claimed in the per-invariant ring since the last level end
+  unsigned long long inv_staged;         // discarded violators staged since the last level end
+  unsigned long long inv_viol_seen;      // viol_count at the last level end (host-written)
+  unsigned long long inv_count[64];      // violators per invariant over the run
 };
 
 // Violating states are rare and terminal, so they go to a small ring: W state words, the
@@ -179,6 +190,12 @@ struct DevCounters {
 // the stored orbit member, which is whichever insert won: the pick is then a choice among orbits.
 static constexpr int VIOL_RING = 1 << 16;     // rows; (W + 3) * 8 bytes each: 2.6 MB for a two-word model
 static constexpr int VIOL_ROW = W + 3;
+// Under "continue" two more rings of the same size and row format follow in the same allocation: the per-invariant ring
+// (the last word of a row is the set of pending invariants the state violates) and the stage of constraint-discarded
+// violators.  The host empties both at every level end.
+static constexpr bool INV_REPORT = M::HAS_INVARIANT_MASK && M::NUM_INVARIANTS > 0;
+__host__ __device__ __forceinline__ uint64_t* inv_ring_of(uint64_t* viol_ring) { return viol_ring + (size_t)VIOL_RING * VIOL_ROW; }
+__host__ __device__ __forceinline__ uint64_t* stage_ring_of(uint64_t* viol_ring) { return viol_ring + (size_t)2 * VIOL_RING * VIOL_ROW; }
 
 struct Params {
   void* table;              // 8-byte slots (one-word models) or 16-byte slots
@@ -213,7 +230,8 @@ static constexpr int INBOX_HEADER = 8;
 // (posted NVLink stores) and its owner polls it locally:
 //   ready[src]   round number src has finished storing rows (and their counts) for, into this rank's inbox
 //   done[dst]    round number dst has finished inserting from ITS inbox (so its buffer of that round may be reused)
-//   board[r][8]  rank r's level summary {level id, new states, violations, store tail, generated, fail, deadlocks, -}
+//   board[r][8]  rank r's level summary {level id, new states, violations, store tail, generated, fail, deadlocks,
+//                pending invariants violated at this level}
 // All counters are monotonic over the life of the context (never reset), so no reset can race with a peer.
 static constexpr int SYNC_WORDS = 256;
 static constexpr int SYNC_READY = 0, SYNC_DONE = 8, SYNC_BOARD = 16, BOARD_WORDS = 8;
@@ -225,6 +243,45 @@ __device__ __forceinline__ unsigned lane_id() {
 }
 __device__ __forceinline__ void reds_add64(uint32_t a, unsigned long long v) {     // shared-memory add, no return value
   asm volatile("red.shared.add.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory");
+}
+
+// The per-invariant report of the invariant violators (`member`) among a warp's states under "continue"
+// (k_invariant_report, for the stored states of a level and the staged successors): their violated invariants counted
+// with one atomic per warp and invariant, and a row in the per-invariant ring for each one that violates an invariant
+// still pending.  Called by all 32 lanes of a warp at a converged point.
+__device__ __noinline__ void record_invariants(DevCounters* ctr, uint64_t* viol_ring, const State& s, uint64_t meta, uint64_t fp,
+                                               bool member) {
+  if (!INV_REPORT || !ctr->inv_on) return;
+  const unsigned active = 0xffffffffu, lane = lane_id();
+  const int leader = 0;
+  const uint64_t m = member ? M::violated_invariants(s) : 0;
+  uint64_t all = (uint64_t)__reduce_or_sync(active, (unsigned)m) | (uint64_t)__reduce_or_sync(active, (unsigned)(m >> 32)) << 32;
+  while (all) {
+    const int i = __ffsll((long long)all) - 1;
+    all &= all - 1;
+    const unsigned who = __ballot_sync(active, (m >> i) & 1);
+    if ((int)lane == leader) atomicAdd(&ctr->inv_count[i], (unsigned long long)__popc(who));
+  }
+  const uint64_t mine = m & ctr->inv_pending;         // (constant while a kernel runs: the host writes it between levels)
+  const unsigned writers = __ballot_sync(active, mine != 0);
+  if (!writers) return;
+  const uint64_t fresh = (uint64_t)__reduce_or_sync(active, (unsigned)mine) |
+                         (uint64_t)__reduce_or_sync(active, (unsigned)(mine >> 32)) << 32;
+  unsigned long long base = 0;
+  if ((int)lane == leader) {
+    atomicOr(&ctr->inv_new, (unsigned long long)fresh);
+    base = atomicAdd(&ctr->inv_rows, (unsigned long long)__popc(writers));
+  }
+  base = __shfl_sync(active, base, leader);
+  if (!mine) return;
+  const unsigned long long slot = base + __popc(writers & ((1u << lane) - 1));
+  if (slot >= (unsigned long long)VIOL_RING) return;
+  uint64_t* row = inv_ring_of(viol_ring) + slot * VIOL_ROW;
+#pragma unroll
+  for (int k = 0; k < W; ++k) row[k] = s.w[k];
+  row[W] = meta;
+  row[W + 1] = fp;
+  row[W + 2] = mine;
 }
 
 // Out of line (rare, terminal), so it takes the two pointers it uses by value: a `const Params&` argument would make
@@ -239,6 +296,20 @@ __device__ __noinline__ void record_violation(DevCounters* ctr, uint64_t* viol_r
   row[W] = meta;
   row[W + 1] = fp;
   row[W + 2] = inv;
+}
+
+// A successor a CONSTRAINT discards is not stored, so under "continue" a violating one is staged (W words, parent word,
+// fingerprint) for k_invariant_report.  Kept apart from record_invariants: evaluating every invariant here would
+// raise the register use of this call, and with it the spills of the expand kernel that inserts successors itself.
+__device__ __noinline__ void stage_violator(DevCounters* ctr, uint64_t* viol_ring, const State& s, uint64_t meta, uint64_t fp) {
+  if (!INV_REPORT || !ctr->inv_on) return;
+  const unsigned long long slot = atomicAdd(&ctr->inv_staged, 1ull);
+  if (slot >= (unsigned long long)VIOL_RING) return;
+  uint64_t* row = stage_ring_of(viol_ring) + slot * VIOL_ROW;
+#pragma unroll
+  for (int k = 0; k < W; ++k) row[k] = s.w[k];
+  row[W] = meta;
+  row[W + 1] = fp;
 }
 
 // ----------------------------------------------------------------------------------------
@@ -381,7 +452,10 @@ __device__ __forceinline__ void insert_row(const Params& p, const State& s, uint
       // so that (rare) case is handled here.  New in-model states are checked by k_invariants (K3).
       if (M::NUM_INVARIANTS > 0) {
         int inv = M::first_violated_invariant(s);
-        if (inv >= 0) record_violation(p.ctr, p.viol_ring, s, meta, f.id.fp, (uint64_t)inv);
+        if (inv >= 0) {
+          record_violation(p.ctr, p.viol_ring, s, meta, f.id.fp, (uint64_t)inv);
+          stage_violator(p.ctr, p.viol_ring, s, meta, f.id.fp);
+        }
       }
     }
   }
@@ -1029,6 +1103,7 @@ __global__ void k_publish_level(Params p, uint64_t level_id, uint64_t prev_tail)
     e[4] = p.ctr->generated;
     e[5] = p.ctr->fail;
     e[6] = p.ctr->deadlocks;
+    e[7] = p.ctr->inv_new;
     __threadfence_system();
     st_release_sys(e, level_id);
   }
@@ -1111,6 +1186,43 @@ __global__ void __launch_bounds__(256) k_invariants(Params p, uint64_t first, co
   }
 }
 
+// K3 of a "continue" run, after k_invariants: the per-invariant report of the level's violators -- its new states and the
+// discarded successors the inserts staged.  A level without violators (the violator count did not move since the last
+// level end) returns at once, so k_invariants itself is unchanged; a level with some checks its new states a second
+// time, in whole rounds of 32 (the last one padded) so that record_invariants is called by converged warps.
+__global__ void __launch_bounds__(256) k_invariant_report(Params p, uint64_t first, const unsigned long long* end_ptr) {
+  if (!INV_REPORT || !p.ctr->inv_on || p.ctr->viol_count == p.ctr->inv_viol_seen) return;
+  uint64_t end = (uint64_t)*end_ptr;
+  if (end - p.store_base > p.max_states) end = p.store_base + p.max_states;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t end_round = first + ((end - first + 31) & ~31ull);
+  for (uint64_t i = first + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < end_round; i += stride) {
+    State s;
+    bool member = false;
+    if (i < end) {
+      const uint64_t* src = p.store + (i & p.store_mask) * W;
+#pragma unroll
+      for (int k = 0; k < W; ++k) s.w[k] = __ldcs(src + k);
+      member = M::first_violated_invariant(s) >= 0;
+    }
+    if (__ballot_sync(0xffffffffu, member))
+      record_invariants(p.ctr, p.viol_ring, s, member ? p.parent[i & p.store_mask] : 0, member ? state_fp(s) : 0, member);
+  }
+  const uint64_t staged = p.ctr->inv_staged < (uint64_t)VIOL_RING ? p.ctr->inv_staged : (uint64_t)VIOL_RING;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < ((staged + 31) & ~31ull); j += stride) {
+    State s;
+    uint64_t meta = 0, fp = 0;
+    if (j < staged) {
+      const uint64_t* row = stage_ring_of(p.viol_ring) + j * VIOL_ROW;
+#pragma unroll
+      for (int k = 0; k < W; ++k) s.w[k] = row[k];
+      meta = row[W];
+      fp = row[W + 1];
+    }
+    record_invariants(p.ctr, p.viol_ring, s, meta, fp, j < staged);
+  }
+}
+
 // -recover: the set is not part of a checkpoint; it is rebuilt from the stored states (one insert each)
 __global__ void __launch_bounds__(256) k_rebuild(Params p, const uint64_t* states, uint64_t n) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -1152,6 +1264,17 @@ __global__ void k_fpset_put(void* table, uint64_t bucket_mask, const uint64_t* f
 struct LaunchRec {
   int kind;  // 0 expand, 1 insert, 2 other
   cudaEvent_t a, b;
+};
+
+// The report of one invariant (kmc_invariant_reports): its first violating level, the violators there, and the pick
+// among them by build_trace's rule with its trace.  `words` is empty when every violator of that level fell beyond
+// the per-invariant ring.
+struct InvReport {
+  int32_t inv = -1;
+  uint64_t level = 0, first_count = 0, fp = 0, meta = 0;
+  std::vector<uint64_t> words;
+  std::vector<std::vector<uint64_t>> trace;
+  std::vector<uint32_t> actions;
 };
 
 struct Engine {
@@ -1219,6 +1342,12 @@ struct Engine {
   std::vector<uint32_t> trace_actions;
   std::vector<uint64_t> viol_words;     // the offending state itself and its parent/action word
   uint64_t viol_meta = 0;
+  // per-invariant report of a "continue" run, in the order found; complete = 0 after a recover (it then covers only
+  // the levels searched since)
+  std::vector<InvReport> inv_reports;
+  uint64_t inv_pending = 0;
+  std::vector<uint64_t> inv_count = std::vector<uint64_t>(64, 0);     // violators per invariant (the counters)
+  bool inv_complete = true;
   bool ran = false;
   // the level cursor: the states [level_first, level_first + level_count) form BFS level `level`, the one expanded
   // next (level 0: nothing inserted yet)
@@ -1417,9 +1546,22 @@ static int engine_alloc(Engine& E) {
   // the expand kernel keeps its state tile, the successor stage and the pair list in > 48 KB of dynamic shared memory
   CK(cudaFuncSetAttribute(k_expand, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EXPAND_SMEM_BYTES));
   CK(cudaMalloc(&E.ctr, sizeof(DevCounters)));
-  CK(cudaMalloc(&E.viol_ring, (size_t)VIOL_RING * VIOL_ROW * 8));
+  CK(cudaMalloc(&E.viol_ring, (size_t)(INV_REPORT && E.cont ? 3 : 1) * VIOL_RING * VIOL_ROW * 8));   // (see inv_ring_of)
   CK(cudaEventCreate(&E.ev_begin));
   CK(cudaEventCreate(&E.ev_end));
+  return KMC_OK;
+}
+
+static uint64_t all_invariants() { return M::NUM_INVARIANTS >= 64 ? ~0ull : (1ull << M::NUM_INVARIANTS) - 1; }
+
+// The per-invariant report starts afresh (every invariant pending) and, under "continue", the recorder is switched on.
+static int inv_begin(Engine& E, bool complete) {
+  const bool on = INV_REPORT && E.cont;
+  E.inv_reports.clear();
+  E.inv_pending = on ? all_invariants() : 0;
+  E.inv_complete = complete;
+  const unsigned long long w[6] = {on ? 1ull : 0ull, E.inv_pending, 0, 0, 0, 0};   // inv_on .. inv_viol_seen
+  CK(cudaMemcpyAsync(&E.ctr->inv_on, w, sizeof(w), cudaMemcpyHostToDevice, E.stream));
   return KMC_OK;
 }
 
@@ -1445,9 +1587,10 @@ static int engine_reset(Engine& E) {
     std::lock_guard<std::mutex> g(E.mu);
     std::fill(E.site_generated.begin(), E.site_generated.end(), 0);
     std::fill(E.action_distinct.begin(), E.action_distinct.end(), 0);
+    std::fill(E.inv_count.begin(), E.inv_count.end(), 0);
     E.coverage_complete = true;
   }
-  return KMC_OK;
+  return inv_begin(E, true);
 }
 
 // The stats and coverage that come from the device counters (the caller holds E.mu).  kmc_run clamps distinct to
@@ -1464,6 +1607,7 @@ static void publish(Engine& E, const DevCounters& h, bool clamp) {
   st.max_states = E.max_states;
   E.site_generated.assign(h.site_generated, h.site_generated + M::NUM_SITES);
   E.action_distinct.assign(h.action_distinct, h.action_distinct + M::NUM_ACTIONS);
+  E.inv_count.assign(h.inv_count, h.inv_count + 64);
 }
 
 static int read_counters(Engine& E, DevCounters* h) {
@@ -1527,7 +1671,9 @@ static int launch_invariants(Engine& E, uint64_t first, uint64_t count_bound) {
   if (M::NUM_INVARIANTS == 0) return KMC_OK;
   Params p = E.params();
   TimedLaunch t(E, 2);
-  k_invariants<<<grid_for(E, std::max<uint64_t>(count_bound, 1), 256, 8), 256, 0, E.stream>>>(p, first, &E.ctr->store_tail);
+  const int grid = grid_for(E, std::max<uint64_t>(count_bound, 1), 256, 8);
+  k_invariants<<<grid, 256, 0, E.stream>>>(p, first, &E.ctr->store_tail);
+  if (INV_REPORT && E.cont) k_invariant_report<<<grid, 256, 0, E.stream>>>(p, first, &E.ctr->store_tail);
   CK(cudaGetLastError());
   return KMC_OK;
 }
@@ -1752,6 +1898,29 @@ static int read_checkpoint(Engine& E, DevCounters* h) {
 // Picks the violator with the smallest fingerprint (deadlocks, which belong to the level being
 // expanded, before invariant violations of the next level) and walks its parent links back to an
 // initial state.  `level` is the level being expanded (0 for the init insert).
+// The trace of a violator (its words and parent word) back to an initial state along the parent links, through the host
+// spill.  A parent on another rank ends the walk (multi_run walks across the ranks).
+static int walk_trace(Engine& E, const uint64_t* words, uint64_t meta, std::vector<std::vector<uint64_t>>& trace,
+                      std::vector<uint32_t>& actions) {
+  std::vector<std::vector<uint64_t>> rev;
+  std::vector<uint32_t> rev_act;
+  rev.push_back(std::vector<uint64_t>(words, words + W));
+  rev_act.push_back((uint32_t)(meta >> 56));
+  uint64_t guard = 0;
+  while ((meta & 0x0000FFFFFFFFFFFFull) != NO_PARENT && guard++ < 100000) {
+    uint64_t idx = meta & IDX_MASK;
+    uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
+    if (prank != E.rank || idx - E.store_base >= E.max_states && idx >= E.store_base) break;  // parent lives on another rank
+    std::vector<uint64_t> st(W);
+    if (int rc = read_range(E, idx, 1, st.data(), &meta)) return rc;
+    rev.push_back(st);
+    rev_act.push_back((uint32_t)(meta >> 56));
+  }
+  trace.assign(rev.rbegin(), rev.rend());
+  actions.assign(rev_act.rbegin(), rev_act.rend());
+  return KMC_OK;
+}
+
 static int build_trace(Engine& E, const DevCounters& h, uint64_t level) {
   uint64_t n = std::min<uint64_t>(h.viol_count, VIOL_RING);
   if (n == 0) return KMC_OK;
@@ -1765,31 +1934,52 @@ static int build_trace(Engine& E, const DevCounters& h, uint64_t level) {
     if (r_dead != b_dead) { if (r_dead) best = r; continue; }
     if (r[W + 1] < best[W + 1] || (r[W + 1] == best[W + 1] && r[W] < best[W])) best = r;
   }
-  std::vector<std::vector<uint64_t>> rev;
-  std::vector<uint32_t> rev_act;
-  uint64_t meta = best[W];
   E.viol_words.assign(best, best + W);
-  E.viol_meta = meta;
-  rev.push_back(std::vector<uint64_t>(best, best + W));
-  rev_act.push_back((uint32_t)(meta >> 56));
-  uint64_t guard = 0;
-  while ((meta & 0x0000FFFFFFFFFFFFull) != NO_PARENT && guard++ < 100000) {
-    uint64_t idx = meta & IDX_MASK;
-    uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
-    if (prank != E.rank || idx - E.store_base >= E.max_states && idx >= E.store_base) break;  // parent lives on another rank
-    std::vector<uint64_t> st(W);
-    if (int rc = read_range(E, idx, 1, st.data(), &meta)) return rc;
-    rev.push_back(st);
-    rev_act.push_back((uint32_t)(meta >> 56));
-  }
-  E.trace.assign(rev.rbegin(), rev.rend());
-  E.trace_actions.assign(rev_act.rbegin(), rev_act.rend());
+  E.viol_meta = best[W];
+  if (int rc = walk_trace(E, best, best[W], E.trace, E.trace_actions)) return rc;
   bool dead = best[W + 2] == ~0ull;
   E.viol.kind = dead ? KMC_RESULT_DEADLOCK : KMC_RESULT_INVARIANT;
   E.viol.invariant = dead ? -1 : (int32_t)best[W + 2];
   E.viol.level = dead ? level : level + 1;
   E.viol.trace_len = E.trace.size();
   E.viol.fingerprint = best[W + 1];
+  return KMC_OK;
+}
+
+// Level end of a "continue" run: every pending invariant that a state of level `level` violates (`fresh`: the inv_new
+// words of the ranks, ORed) is reported -- its violators at that level (before it, it had none) and its pick from the
+// per-invariant ring by build_trace's rule (smallest fingerprint, then smallest parent word).  `walk`: walk the pick's
+// trace now (one rank; multi_run walks across the ranks).  Then those invariants stop being pending and the rings empty.
+// A level with more discarded violators than the stage holds makes the report incomplete.
+static int collect_invariants(Engine& E, const DevCounters& h, uint64_t level, uint64_t fresh, bool walk) {
+  fresh &= E.inv_pending;
+  if (h.inv_staged > (uint64_t)VIOL_RING) E.inv_complete = false;
+  const uint64_t n = fresh ? std::min<uint64_t>(h.inv_rows, VIOL_RING) : 0;
+  std::vector<uint64_t> ring(n * VIOL_ROW);
+  if (n) CK(cudaMemcpy(ring.data(), inv_ring_of(E.viol_ring), ring.size() * 8, cudaMemcpyDeviceToHost));
+  for (uint64_t b = fresh; b; b &= b - 1) {
+    InvReport r;
+    r.inv = __builtin_ctzll(b);
+    r.level = level;
+    r.first_count = h.inv_count[r.inv];
+    const uint64_t* best = nullptr;
+    for (uint64_t k = 0; k < n; ++k) {
+      const uint64_t* row = ring.data() + k * VIOL_ROW;
+      if (!((row[W + 2] >> r.inv) & 1)) continue;
+      if (!best || row[W + 1] < best[W + 1] || (row[W + 1] == best[W + 1] && row[W] < best[W])) best = row;
+    }
+    if (best) {
+      r.fp = best[W + 1];
+      r.meta = best[W];
+      r.words.assign(best, best + W);
+      if (walk)
+        if (int rc = walk_trace(E, best, best[W], r.trace, r.actions)) return rc;
+    }
+    E.inv_reports.push_back(std::move(r));
+  }
+  E.inv_pending &= ~fresh;
+  const unsigned long long w[5] = {E.inv_pending, 0, 0, 0, h.viol_count};   // inv_pending .. inv_viol_seen
+  CK(cudaMemcpyAsync(&E.ctr->inv_pending, w, sizeof(w), cudaMemcpyHostToDevice, E.stream));
   return KMC_OK;
 }
 
@@ -1825,6 +2015,7 @@ static int end_level(Engine& E, uint64_t inv_bound, bool shard, DevCounters& h) 
     else E.stats.queue = E.level_count;
   }
   if (h.viol_count && E.viol.kind == KMC_RESULT_OK && (shard || !h.fail)) build_trace(E, h, level);
+  if (INV_REPORT && E.cont && (shard || !h.fail)) return collect_invariants(E, h, level + 1, h.inv_new, true);
   return KMC_OK;
 }
 
@@ -1844,6 +2035,7 @@ static int engine_run(Engine& E) {
   if (!E.recover_dir.empty()) {
     // -recover: continue from the level boundary a checkpoint was written at
     if ((rc = read_checkpoint(E, &h))) return rc;
+    if ((rc = inv_begin(E, false))) return rc;
   } else {
     if ((rc = seed_init(E))) return rc;
     if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, M::NUM_INIT))) return rc;
@@ -2069,6 +2261,56 @@ int kmcm_violation_record(const kmcm_ctx* c, uint64_t* words, size_t cap_words, 
   memcpy(words, E.viol_words.data(), W * 8);
   *parent_meta = E.viol_meta;
   return KMC_OK;
+}
+
+// the reports of a "continue" run, ordered by (level, invariant); the multi-process driver's ranks (world > 1 without
+// "gpus") each see only their own violators and report nothing
+static bool inv_reports_readable(const kmcm_ctx* c, int* rc) {
+  *rc = !M::HAS_INVARIANT_MASK ? KMC_E_BADARG : (c->ranks.empty() && E.world > 1) || (!E.ran && E.level == 0) ? KMC_E_STATE : KMC_OK;
+  return *rc == KMC_OK;
+}
+static std::vector<const InvReport*> inv_reports_sorted(const Engine& e) {
+  std::vector<const InvReport*> v;
+  for (const InvReport& r : e.inv_reports) v.push_back(&r);
+  std::sort(v.begin(), v.end(), [](const InvReport* a, const InvReport* b) { return a->level != b->level ? a->level < b->level : a->inv < b->inv; });
+  return v;
+}
+
+int kmcm_invariant_reports(const kmcm_ctx* c, kmc_invariant_report_t* out, size_t cap, size_t* n, int32_t* complete) {
+  if (!c || !n || !complete || (!out && cap)) return KMC_E_BADARG;
+  int rc;
+  if (!inv_reports_readable(c, &rc)) return rc;
+  std::lock_guard<std::mutex> g(E.mu);
+  const std::vector<const InvReport*> v = inv_reports_sorted(E);
+  *n = v.size();
+  *complete = E.inv_complete ? 1 : 0;
+  for (size_t k = 0; k < v.size() && k < cap; ++k) {
+    kmc_invariant_report_t& o = out[k];
+    memset(&o, 0, sizeof(o));
+    o.invariant = v[k]->inv;
+    o.level = v[k]->level;
+    o.violators_first_level = v[k]->first_count;
+    o.violators = E.inv_count[v[k]->inv];
+    o.trace_len = v[k]->trace.size();
+    o.fingerprint = v[k]->fp;
+  }
+  return KMC_OK;
+}
+
+int kmcm_invariant_trace_state(const kmcm_ctx* c, int32_t invariant, uint32_t i, uint64_t* buf, size_t cap_words,
+                               uint32_t* action_id) {
+  if (!c || !buf || cap_words < (size_t)W) return KMC_E_BADARG;
+  int rc;
+  if (!inv_reports_readable(c, &rc)) return rc;
+  std::lock_guard<std::mutex> g(E.mu);
+  for (const InvReport& r : E.inv_reports) {
+    if (r.inv != invariant) continue;
+    if (i >= r.trace.size()) return KMC_E_BADARG;
+    memcpy(buf, r.trace[i].data(), W * 8);
+    if (action_id) *action_id = r.actions[i];
+    return KMC_OK;
+  }
+  return KMC_E_BADARG;
 }
 
 // states and / or parent words [first, first + count) by global index
@@ -2378,6 +2620,13 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
     if ((rc = read_counters(E, &h))) return rc;
     build_trace(E, h, E.level - 1);
   }
+  // the invariants first violated at this level on any rank stop being pending on every rank
+  uint64_t fresh = 0;
+  for (uint32_t r = 0; r < E.world; ++r) fresh |= E.board_host[(size_t)r * BOARD_WORDS + 7];
+  if (INV_REPORT && E.cont) {
+    DevCounters h;
+    if ((rc = read_counters(E, &h)) || (rc = collect_invariants(E, h, E.level, fresh, false))) return rc;
+  }
   return fail_to_error(mine[5]);
 }
 
@@ -2473,6 +2722,33 @@ static int multi_create(kmcm_ctx* c, const char* options_json, int gpus) {
   }
   A.world = (uint32_t)gpus;
   return KMC_OK;
+}
+
+// The trace of a violator found on some rank, following the parent links from store to store.
+static void walk_ranks(kmcm_ctx* c, const std::vector<uint64_t>& words, uint64_t meta, std::vector<std::vector<uint64_t>>& trace,
+                       std::vector<uint32_t>& actions) {
+  const size_t n = c->ranks.size();
+  std::vector<std::vector<uint64_t>> rev;
+  std::vector<uint32_t> rev_act;
+  rev.push_back(words);
+  rev_act.push_back((uint32_t)(meta >> 56));
+  uint64_t guard = 0;
+  while ((meta & 0x0000FFFFFFFFFFFFull) != NO_PARENT && guard++ < 100000) {
+    const uint64_t idx = meta & IDX_MASK;
+    const uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
+    if (prank >= n) break;
+    const Engine& P = c->ranks[prank]->e;
+    if (idx >= P.max_states) break;
+    std::vector<uint64_t> sw(W);
+    if (cudaSetDevice(P.device) != cudaSuccess ||
+        cudaMemcpy(sw.data(), P.store + idx * W, W * 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(&meta, P.parent + idx, 8, cudaMemcpyDeviceToHost) != cudaSuccess)
+      break;
+    rev.push_back(sw);
+    rev_act.push_back((uint32_t)(meta >> 56));
+  }
+  trace.assign(rev.rbegin(), rev.rend());
+  actions.assign(rev_act.rbegin(), rev_act.rend());
 }
 
 struct RankOutcome {
@@ -2590,33 +2866,45 @@ static int multi_run(kmcm_ctx* c) {
     if (R.viol.fingerprint < best->viol.fingerprint) best = &R;
   }
   if (best && !rc) {
-    std::vector<std::vector<uint64_t>> rev;
-    std::vector<uint32_t> rev_act;
-    uint64_t meta = best->viol_meta;
-    rev.push_back(best->viol_words);
-    rev_act.push_back((uint32_t)(meta >> 56));
-    uint64_t guard = 0;
-    while ((meta & 0x0000FFFFFFFFFFFFull) != NO_PARENT && guard++ < 100000) {
-      const uint64_t idx = meta & IDX_MASK;
-      const uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
-      if (prank >= n) break;
-      const Engine& P = c->ranks[prank]->e;
-      if (idx >= P.max_states) break;
-      std::vector<uint64_t> sw(W);
-      if (cudaSetDevice(P.device) != cudaSuccess ||
-          cudaMemcpy(sw.data(), P.store + idx * W, W * 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
-          cudaMemcpy(&meta, P.parent + idx, 8, cudaMemcpyDeviceToHost) != cudaSuccess)
-        break;
-      rev.push_back(sw);
-      rev_act.push_back((uint32_t)(meta >> 56));
-    }
-    A.trace.assign(rev.rbegin(), rev.rend());
-    A.trace_actions.assign(rev_act.rbegin(), rev_act.rend());
+    walk_ranks(c, best->viol_words, best->viol_meta, A.trace, A.trace_actions);
     A.viol = best->viol;
     A.viol.trace_len = A.trace.size();
     A.viol_words = best->viol_words;
     A.viol_meta = best->viol_meta;
   }
+  // per-invariant report: every rank reported the same invariants at the same levels (they share the board); the
+  // violators are summed and the pick is the rule's pick among the ranks' picks
+  A.inv_reports.clear();
+  A.inv_complete = true;
+  std::fill(A.inv_count.begin(), A.inv_count.end(), 0);
+  for (size_t r = 0; r < n; ++r) {
+    const Engine& R = c->ranks[r]->e;
+    A.inv_complete = A.inv_complete && R.inv_complete;
+    for (size_t i = 0; i < A.inv_count.size(); ++i) A.inv_count[i] += R.inv_count[i];
+    for (const InvReport& x : R.inv_reports) {
+      InvReport* y = nullptr;
+      for (InvReport& a : A.inv_reports)
+        if (a.inv == x.inv) y = &a;
+      if (!y || x.level < y->level) {
+        if (!y) {
+          A.inv_reports.emplace_back();
+          y = &A.inv_reports.back();
+        }
+        *y = x;
+        continue;
+      }
+      if (x.level > y->level) continue;
+      y->first_count += x.first_count;
+      if (!x.words.empty() && (y->words.empty() || x.fp < y->fp || (x.fp == y->fp && x.meta < y->meta))) {
+        y->fp = x.fp;
+        y->meta = x.meta;
+        y->words = x.words;
+      }
+    }
+  }
+  if (!rc)
+    for (InvReport& a : A.inv_reports)
+      if (!a.words.empty()) walk_ranks(c, a.words, a.meta, a.trace, a.actions);
   A.ran = true;
   return rc;
 }

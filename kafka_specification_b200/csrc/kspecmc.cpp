@@ -33,6 +33,8 @@ struct kmc_ctx {
   int (*copy_states)(const kmcm_ctx*, uint64_t, uint64_t, uint64_t*) = nullptr;
   int (*copy_parents)(const kmcm_ctx*, uint64_t, uint64_t, uint64_t*) = nullptr;
   int (*violation_record)(const kmcm_ctx*, uint64_t*, size_t, uint64_t*) = nullptr;
+  int (*invariant_reports)(const kmcm_ctx*, kmc_invariant_report_t*, size_t, size_t*, int32_t*) = nullptr;
+  int (*invariant_trace_state)(const kmcm_ctx*, int32_t, uint32_t, uint64_t*, size_t, uint32_t*) = nullptr;
   const char* (*strerror_)(const kmcm_ctx*, int) = nullptr;
   int (*fpset_put)(kmcm_ctx*, const uint64_t*, size_t, uint8_t*) = nullptr;
   int (*fpset_contains)(kmcm_ctx*, const uint64_t*, size_t, uint8_t*) = nullptr;
@@ -86,6 +88,8 @@ int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out) {
             bind(c, c->violation, "kmcm_violation") &&
             bind(c, c->trace_state, "kmcm_trace_state") && bind(c, c->copy_states, "kmcm_copy_states") &&
             bind(c, c->copy_parents, "kmcm_copy_parents") && bind(c, c->violation_record, "kmcm_violation_record") &&
+            bind(c, c->invariant_reports, "kmcm_invariant_reports") &&
+            bind(c, c->invariant_trace_state, "kmcm_invariant_trace_state") &&
             bind(c, c->strerror_, "kmcm_strerror") && bind(c, c->fpset_put, "kmcm_fpset_put") &&
             bind(c, c->fpset_contains, "kmcm_fpset_contains") && bind(c, c->fpset_size, "kmcm_fpset_size") &&
             bind(c, c->shard_begin, "kmcm_shard_begin") && bind(c, c->shard_buffers, "kmcm_shard_buffers") &&
@@ -133,6 +137,12 @@ int kmc_trace_state(const kmc_ctx* c, uint32_t i, uint64_t* buf, size_t cap, uin
 int kmc_copy_states(const kmc_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) { FWD(copy_states, first, count, buf); }
 int kmc_copy_parents(const kmc_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) { FWD(copy_parents, first, count, buf); }
 int kmc_violation_record(const kmc_ctx* c, uint64_t* words, size_t cap, uint64_t* meta) { FWD(violation_record, words, cap, meta); }
+int kmc_invariant_reports(const kmc_ctx* c, kmc_invariant_report_t* out, size_t cap, size_t* n, int32_t* complete) {
+  FWD(invariant_reports, out, cap, n, complete);
+}
+int kmc_invariant_trace_state(const kmc_ctx* c, int32_t inv, uint32_t i, uint64_t* buf, size_t cap, uint32_t* a) {
+  FWD(invariant_trace_state, inv, i, buf, cap, a);
+}
 int kmc_fpset_put(kmc_ctx* c, const uint64_t* fps, size_t n, uint8_t* seen) { FWD(fpset_put, fps, n, seen); }
 int kmc_fpset_contains(kmc_ctx* c, const uint64_t* fps, size_t n, uint8_t* out) { FWD(fpset_contains, fps, n, out); }
 int kmc_fpset_size(const kmc_ctx* c, uint64_t* out) { FWD(fpset_size, out); }

@@ -22,6 +22,7 @@ from .compiler import Block, Closure, Lowerer, Marker, Thunk, render
 from .svals import LowerError, SLazy, is_atom_const, is_const, is_int_const
 
 LOWERING_VERSION = 3
+MAX_MASK_INVARIANTS = 64       # violated_invariants() returns one bit per INVARIANT
 
 
 @dataclass
@@ -44,6 +45,7 @@ class LoweredModel:
     variables: list[str] = field(default_factory=list)
     sites: list[dict] = field(default_factory=list)     # per emit site: {"action": index into actions, -1 = trap only}
     init: dict = field(default_factory=dict)            # the initial predicate: name, module and source span
+    invariants_header: str = ""                         # invariants.h: violated_invariants(), compiled after the header
 
 
     def meta(self) -> dict:
@@ -622,16 +624,23 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
         site_groups.append(cur)
     max_fanout = lw.emit_sites
 
-    # invariants
+    # invariants.  Each one ends in a top-level `return i` statement; violated_invariants() is the same tree with those
+    # statements setting bit i instead, so that every invariant is evaluated.
     lw.begin_function()
+    inv_exits: dict[int, str] = {}          # index in the body's children -> the statement of the mask form
     for i, inv in enumerate(cfg.invariants):
         idf, ictx = lw.named_def(inv)
         c = lw.ev_bool(idf.body, ictx, idf.module, {})
         if c is False:
             lw.cg.emit(f"return {i};")
+            inv_exits[len(lw.cg.body.children) - 1] = f"m |= 1ull << {i};"
         elif c is not True:
             lw.cg.emit(f"if (!({c.s})) return {i};")
+            inv_exits[len(lw.cg.body.children) - 1] = f"if (!({c.s})) m |= 1ull << {i};"
+        if len(lw.cg.stack) != 1:
+            raise LowerError(f"internal: invariant {inv} left a block open")
     inv_lines = lw.prologue + render(lw.cg.body.children, 1)
+    mask_lines = lw.prologue + render([inv_exits.get(k, n) for k, n in enumerate(lw.cg.body.children)], 1)
 
     # constraints
     lw.begin_function()
@@ -772,10 +781,23 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     parts.append("}  // namespace kmc_model")
     header = "\n".join(parts) + "\n"
 
+    # invariants.h, included after model.h: the invariants as a bit mask (up to 64 of them)
+    if len(cfg.invariants) <= MAX_MASK_INVARIANTS:
+        mask_fn = (["/* bit i set iff INVARIANT i of the cfg is false: first_violated_invariant with every invariant evaluated */",
+                    "KMC_HD uint64_t violated_invariants(const State& s) {"] + unpack + ["  uint64_t m = 0;"] + mask_lines +
+                   ["  return m;", "}"])
+    else:
+        mask_fn = [f"/* {len(cfg.invariants)} INVARIANTs do not fit a 64-bit mask: no per-invariant report for this model */",
+                   "KMC_HD uint64_t violated_invariants(const State&) { return 0; }"]
+    invariants_header = "\n".join([f"// generated by the lowering for {name}: the companion of model.h", "namespace kmc_model {",
+                                   f"static constexpr bool HAS_INVARIANT_MASK = {'true' if len(cfg.invariants) <= MAX_MASK_INVARIANTS else 'false'};",
+                                   *mask_fn, "}  // namespace kmc_model"]) + "\n"
+
     return LoweredModel(
         name=name, module=module, header=header, layout=lay.describe(), words=lay.words,
         state_bits=lay.bits, init_states=init_words, actions=lw.actions or [{"name": "Next", "module": module}],
         invariants=list(cfg.invariants), constraints=list(cfg.constraints),
         check_deadlock=cfg.check_deadlock, max_fanout=max(1, max_fanout), warnings=lw.warnings,
         digest=body_digest, lowerer=lw, variables=list(lw.variables),
-        sites=[{"action": a} for a in site_action], init=_init_info(lw, init_e, module))
+        sites=[{"action": a} for a in site_action], init=_init_info(lw, init_e, module),
+        invariants_header=invariants_header)

@@ -52,6 +52,11 @@ class Violation(ctypes.Structure):
                 ("trace_len", ctypes.c_uint64), ("fingerprint", ctypes.c_uint64)]
 
 
+class InvariantReport(ctypes.Structure):
+    _fields_ = [("invariant", ctypes.c_int32), ("level", ctypes.c_uint64), ("violators_first_level", ctypes.c_uint64),
+                ("violators", ctypes.c_uint64), ("trace_len", ctypes.c_uint64), ("fingerprint", ctypes.c_uint64)]
+
+
 class ModelInfo(ctypes.Structure):
     _fields_ = [("words", ctypes.c_int32), ("state_bits", ctypes.c_int32), ("num_actions", ctypes.c_int32),
                 ("num_invariants", ctypes.c_int32), ("num_init", ctypes.c_int32), ("max_fanout", ctypes.c_int32),
@@ -93,6 +98,10 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.kmc_copy_states.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp]
     lib.kmc_copy_parents.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp]
     lib.kmc_violation_record.argtypes = [vp, u64p, ctypes.c_size_t, u64p]
+    lib.kmc_invariant_reports.argtypes = [vp, ctypes.POINTER(InvariantReport), ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t),
+                                          ctypes.POINTER(ctypes.c_int32)]
+    lib.kmc_invariant_trace_state.argtypes = [vp, ctypes.c_int32, ctypes.c_uint32, u64p, ctypes.c_size_t,
+                                              ctypes.POINTER(ctypes.c_uint32)]
     lib.kmc_strerror.argtypes = [vp, ctypes.c_int]
     lib.kmc_strerror.restype = ctypes.c_char_p
     lib.kmc_fpset_put.argtypes = [vp, vp, ctypes.c_size_t, vp]
@@ -117,7 +126,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.kmc_shard_inbox_ptr.argtypes = [vp, ctypes.POINTER(vp)]
     lib.kmc_shard_open_peers_direct.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.c_uint32]
     for fn in ("kmc_create", "kmc_model_info", "kmc_run", "kmc_stats", "kmc_level_widths", "kmc_action_counts", "kmc_coverage",
-               "kmc_violation", "kmc_trace_state", "kmc_copy_states", "kmc_copy_parents", "kmc_violation_record", "kmc_fpset_put", "kmc_fpset_contains",
+               "kmc_violation", "kmc_trace_state", "kmc_copy_states", "kmc_copy_parents", "kmc_violation_record", "kmc_invariant_reports", "kmc_invariant_trace_state", "kmc_fpset_put", "kmc_fpset_contains",
                "kmc_fpset_size", "kmc_shard_begin", "kmc_shard_buffers", "kmc_shard_seed_init", "kmc_shard_expand",
                "kmc_shard_counts", "kmc_shard_reset_cand", "kmc_shard_insert", "kmc_shard_level_done", "kmc_shard_sync",
                "kmc_shard_ipc_handle", "kmc_shard_open_peers", "kmc_shard_seed_p2p", "kmc_shard_expand_p2p",
@@ -360,6 +369,8 @@ class RunResult:
     stats: dict
     violation: dict | None = None
     trace: list[dict] = field(default_factory=list)
+    # with "continue": every violated invariant (Checker.invariant_reports), ordered by (level, cfg index)
+    invariant_violations: list[dict] = field(default_factory=list)
 
 
 class Checker:
@@ -377,6 +388,7 @@ class Checker:
         self.decoder = StateDecoder(self.meta)
         self.ctx = ctypes.c_void_p()
         opts = {("continue" if k == "cont" else k): v for k, v in options.items() if k not in ("p2p", "device_sync")}
+        self.cont = bool(opts.get("continue"))
         rc = self.lib.kmc_create(self.model_lib.encode(), json.dumps(opts).encode(), ctypes.byref(self.ctx))
         if rc != 0:
             msg = self.lib.kmc_strerror(self.ctx, rc).decode() if self.ctx else "kmc_create failed"
@@ -467,6 +479,11 @@ class Checker:
                 "invariant": self.meta["invariants"][v.invariant] if v.kind == 1 else None,
                 "level": int(v.level), "trace_len": int(v.trace_len), "fingerprint": int(v.fingerprint)}
 
+    def _trace_entry(self, i: int, buf, act) -> dict:
+        words = [int(buf[k]) for k in range(self.words)]
+        a = self.meta["actions"][act.value] if (i > 0 and act.value < len(self.meta["actions"])) else None
+        return {"words": words, "action": a, "state": self.decoder.decode(words), "text": self.decoder.text(words)}
+
     def trace(self) -> list[dict]:
         v = self.violation()
         if v is None:
@@ -476,10 +493,30 @@ class Checker:
         act = ctypes.c_uint32()
         for i in range(v["trace_len"]):
             self._check(self.lib.kmc_trace_state(self.ctx, i, buf, self.words, ctypes.byref(act)))
-            words = [int(buf[k]) for k in range(self.words)]
-            a = self.meta["actions"][act.value] if (i > 0 and act.value < len(self.meta["actions"])) else None
-            out.append({"words": words, "action": a, "state": self.decoder.decode(words),
-                        "text": self.decoder.text(words)})
+            out.append(self._trace_entry(i, buf, act))
+        return out
+
+    def invariant_reports(self) -> list[dict]:
+        """Every invariant the last ``continue`` run found violated, ordered by (level, cfg index): ``invariant`` (name),
+        ``index`` (in the cfg), ``level`` (its first violating level), ``violators_first_level``, ``violators``,
+        ``fingerprint``, ``trace_len``, ``trace`` (decoded like ``trace()``: the counterexample ending in the smallest-
+        fingerprint violator of that level) and ``complete`` (False after a recover: only the levels searched since)."""
+        n, complete = ctypes.c_size_t(), ctypes.c_int32()
+        self._check(self.lib.kmc_invariant_reports(self.ctx, None, 0, ctypes.byref(n), ctypes.byref(complete)))
+        reps = (InvariantReport * max(n.value, 1))()
+        self._check(self.lib.kmc_invariant_reports(self.ctx, reps, n.value, ctypes.byref(n), ctypes.byref(complete)))
+        buf = (ctypes.c_uint64 * self.words)()
+        act = ctypes.c_uint32()
+        out = []
+        for r in reps[:n.value]:
+            trace = []
+            for i in range(r.trace_len):
+                self._check(self.lib.kmc_invariant_trace_state(self.ctx, r.invariant, i, buf, self.words, ctypes.byref(act)))
+                trace.append(self._trace_entry(i, buf, act))
+            out.append({"invariant": self.meta["invariants"][r.invariant], "index": int(r.invariant), "level": int(r.level),
+                        "violators_first_level": int(r.violators_first_level), "violators": int(r.violators),
+                        "fingerprint": int(r.fingerprint), "trace_len": int(r.trace_len), "trace": trace,
+                        "complete": bool(complete.value)})
         return out
 
     def run(self, raise_on_error: bool = True) -> RunResult:
@@ -494,9 +531,11 @@ class Checker:
     def result(self) -> RunResult:
         st = self.stats()
         viol = self.violation()
+        # (a model with more than 64 invariants has no per-invariant report)
+        reports = self.invariant_reports() if self.cont and len(self.meta["invariants"]) <= 64 else []
         return RunResult(distinct=st["distinct"], generated=st["generated"], depth=st["depth"], queue=st["queue"],
                          deadlocks=st["deadlocks"], complete=bool(st["complete"]), levels=self.level_widths(),
-                         stats=st, violation=viol, trace=self.trace() if viol else [])
+                         stats=st, violation=viol, trace=self.trace() if viol else [], invariant_violations=reports)
 
     def violation_record(self):
         """(packed words, parent word) of this rank's offending state, or None."""

@@ -13,6 +13,11 @@ kmc_create); ``-workers auto`` = one GPU (the GPU grid replaces TLC's worker thr
 messages in TLC's tool-mode markers (``@!@!@STARTMSG code:class @!@!@`` ... ``@!@!@ENDMSG code @!@!@``).
 ``-coverage N`` prints TLC's action-level coverage table ("distinct:generated" per action) once, at the end of the
 run (also after a violation): TLC repeats it every N minutes, but a search here takes seconds.
+``-continue`` searches past violations and prints one error block per violated invariant, ordered by (first violating
+level, cfg index), each with the counterexample that ends in the smallest-fingerprint violator of that level; the first
+block is the one a run without ``-continue`` prints.  TLC under ``-continue`` prints a trace for every violating state
+it meets (as far as its published behaviour goes: TLC cannot be run here to compare); here it is one per invariant.
+A deadlock found on the way keeps its block and its exit status, ahead of the invariant blocks.
 
 Exit status follows TLC: 0 no error, 12 safety (invariant) violation, 11 deadlock,
 10 assumption failure, 150 spec/config error, 1 runtime failure (no GPU, table full, ...).
@@ -118,6 +123,38 @@ def print_coverage(cov: dict):
         msg(kind, text)
 
 
+def trace_messages(trace: list[dict]) -> list[tuple[str, str, int]]:
+    return [("state", f"State {i + 1}: {action_location(t['action'])}\n{t['text']}\n", 4) for i, t in enumerate(trace)]
+
+
+def invariant_messages(name: str, level: int, trace: list[dict]) -> list[tuple[str, str, int]]:
+    """TLC's error block of one violated invariant: (EC kind, text, class) per message."""
+    if level == 1:
+        head = [("inv_initial", f"Error: Invariant {name} is violated by the initial state:", 1)]
+    else:
+        head = [("inv_behavior", f"Error: Invariant {name} is violated.", 1),
+                ("behavior", "Error: The behavior up to this point is:", 1)]
+    return head + trace_messages(trace)
+
+
+def error_messages(violation: dict | None, trace: list[dict], reports: list[dict]) -> tuple[list[tuple[str, str, int]], int]:
+    """The error blocks of a run and its exit status.  `violation` / `trace`: the run's first violation (RunResult);
+    `reports`: its per-invariant reports under -continue (RunResult.invariant_violations, empty otherwise), whose
+    first block is the one of `violation` when that is an invariant violation."""
+    out, code = [], EXIT_OK
+    if violation and violation["kind"] == "deadlock":
+        out = [("deadlock", "Error: Deadlock reached.", 1), ("behavior", "Error: The behavior up to this point is:", 1)]
+        out += trace_messages(trace)
+        code = EXIT_VIOLATION_DEADLOCK
+    elif violation and not reports:
+        out = invariant_messages(violation["invariant"], violation["level"], trace)
+    for r in sorted(reports, key=lambda r: (r["level"], r["index"])):
+        out += invariant_messages(r["invariant"], r["level"], r["trace"])
+    if code == EXIT_OK and (violation or reports):
+        code = EXIT_VIOLATION_SAFETY
+    return out, code
+
+
 def main(argv=None) -> int:
     a = parse_args(argv if argv is not None else sys.argv[1:])
     spec_path = a.spec[:-4] if a.spec.endswith(".tla") else a.spec
@@ -198,23 +235,10 @@ def main(argv=None) -> int:
         return 1
     n_init = len(model.init_states)
     msg("init_done", f"Finished computing initial states: {n_init} distinct state{'s' if n_init != 1 else ''} generated.")
-    exit_code = EXIT_OK
-    if r.violation:
-        v = r.violation
-        if v["kind"] == "deadlock":
-            msg("deadlock", "Error: Deadlock reached.", 1)
-            exit_code = EXIT_VIOLATION_DEADLOCK
-        elif v["level"] == 1:
-            msg("inv_initial", f"Error: Invariant {v['invariant']} is violated by the initial state:", 1)
-            exit_code = EXIT_VIOLATION_SAFETY
-        else:
-            msg("inv_behavior", f"Error: Invariant {v['invariant']} is violated.", 1)
-            exit_code = EXIT_VIOLATION_SAFETY
-        if v["level"] != 1 or v["kind"] == "deadlock":
-            msg("behavior", "Error: The behavior up to this point is:", 1)
-        for i, t in enumerate(r.trace):
-            msg("state", f"State {i + 1}: {action_location(t['action'])}\n{t['text']}\n", 4)
-    else:
+    blocks, exit_code = error_messages(r.violation, r.trace, r.invariant_violations)
+    for kind, text, cls in blocks:
+        msg(kind, text, cls)
+    if not blocks:
         msg("success", "Model checking completed. No error has been found.\n"
                        "  Estimates of the probability that TLC did not check all reachable states\n"
                        "  because two distinct states had the same fingerprint:")
