@@ -45,6 +45,7 @@
 #include <mutex>
 #include <thread>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "kspecmc.h"
@@ -1266,12 +1267,13 @@ struct LaunchRec {
   cudaEvent_t a, b;
 };
 
-// The report of one invariant (kmc_invariant_reports): its first violating level, the violators there, and the pick
-// among them by build_trace's rule with its trace.  `words` is empty when every violator of that level fell beyond
-// the per-invariant ring.
-struct InvReport {
+// A counterexample: the violator picked at `level` (its words, parent/action word `meta` and set-identity fingerprint)
+// and its trace.  inv = -1 for a deadlock.  The run's violation is one (no `words`: none found yet); so is the report
+// of each invariant under "continue" (kmc_invariant_reports), where `first_count` is the invariant's violators at
+// `level`, its first violating level, and `words` is empty when every one of them fell beyond the per-invariant ring.
+struct Counterexample {
   int32_t inv = -1;
-  uint64_t level = 0, first_count = 0, fp = 0, meta = 0;
+  uint64_t level = 0, fp = 0, meta = 0, first_count = 0;
   std::vector<uint64_t> words;
   std::vector<std::vector<uint64_t>> trace;
   std::vector<uint32_t> actions;
@@ -1337,14 +1339,10 @@ struct Engine {
   std::vector<uint64_t> site_generated = std::vector<uint64_t>(M::NUM_SITES, 0);
   std::vector<uint64_t> action_distinct = std::vector<uint64_t>(M::NUM_ACTIONS, 0);
   bool coverage_complete = true;
-  kmc_violation_t viol{};
-  std::vector<std::vector<uint64_t>> trace;
-  std::vector<uint32_t> trace_actions;
-  std::vector<uint64_t> viol_words;     // the offending state itself and its parent/action word
-  uint64_t viol_meta = 0;
+  Counterexample viol;
   // per-invariant report of a "continue" run, in the order found; complete = 0 after a recover (it then covers only
   // the levels searched since)
-  std::vector<InvReport> inv_reports;
+  std::vector<Counterexample> inv_reports;
   uint64_t inv_pending = 0;
   std::vector<uint64_t> inv_count = std::vector<uint64_t>(64, 0);     // violators per invariant (the counters)
   bool inv_complete = true;
@@ -1575,10 +1573,7 @@ static int engine_reset(Engine& E) {
   E.events_used = 0;
   E.launches.clear();
   E.widths.clear();
-  E.trace.clear();
-  E.trace_actions.clear();
-  memset(&E.viol, 0, sizeof(E.viol));
-  E.viol.invariant = -1;
+  E.viol = Counterexample();
   E.level_first = E.level_count = E.level = 0;
   E.store_base = 0;
   E.host_store.clear();
@@ -1895,62 +1890,84 @@ static int read_checkpoint(Engine& E, DevCounters* h) {
   return KMC_OK;
 }
 
-// Picks the violator with the smallest fingerprint (deadlocks, which belong to the level being
-// expanded, before invariant violations of the next level) and walks its parent links back to an
-// initial state.  `level` is the level being expanded (0 for the init insert).
-// The trace of a violator (its words and parent word) back to an initial state along the parent links, through the host
-// spill.  A parent on another rank ends the walk (multi_run walks across the ranks).
-static int walk_trace(Engine& E, const uint64_t* words, uint64_t meta, std::vector<std::vector<uint64_t>>& trace,
-                      std::vector<uint32_t>& actions) {
-  std::vector<std::vector<uint64_t>> rev;
-  std::vector<uint32_t> rev_act;
-  rev.push_back(std::vector<uint64_t>(words, words + W));
-  rev_act.push_back((uint32_t)(meta >> 56));
-  uint64_t guard = 0;
+// The order of violators, the same for every pick: a deadlock first (it belongs to the level being expanded, before the
+// invariant violations of the next level), then the smaller set-identity fingerprint, then the smaller parent word.
+static std::tuple<bool, uint64_t, uint64_t> violator_key(bool deadlock, uint64_t fp, uint64_t meta) {
+  return {!deadlock, fp, meta};
+}
+// Whether x is the better pick: x has a violator and y none, or x's comes first.
+static bool better(const Counterexample& x, const Counterexample& y) {
+  return !x.words.empty() &&
+         (y.words.empty() || violator_key(x.inv < 0, x.fp, x.meta) < violator_key(y.inv < 0, y.fp, y.meta));
+}
+
+// The first of n ring rows in violator order.  inv < 0: every row of the violator ring, whose last word is the invariant
+// or ~0 for a deadlock.  inv >= 0: the rows of the per-invariant ring whose last word, a set of invariants, holds `inv`;
+// that ring has no deadlocks.  Null when no row qualifies.
+static const uint64_t* pick(const uint64_t* rows, uint64_t n, int inv) {
+  auto key = [inv](const uint64_t* r) { return violator_key(inv < 0 && r[W + 2] == ~0ull, r[W + 1], r[W]); };
+  const uint64_t* best = nullptr;
+  for (const uint64_t* r = rows; r < rows + n * VIOL_ROW; r += VIOL_ROW)
+    if ((inv < 0 || (r[W + 2] >> inv) & 1) && (!best || key(r) < key(best))) best = r;
+  return best;
+}
+
+static void take_row(Counterexample& x, const uint64_t* row) {
+  x.words.assign(row, row + W);
+  x.meta = row[W];
+  x.fp = row[W + 1];
+}
+
+// The trace of x back to an initial state along the parent links, each parent read on its own rank (through that
+// rank's host spill): `ranks` is {&E} for one rank, or every rank of a "gpus" context.  A parent on a rank not in
+// `ranks` ends the walk (the multi-process driver's ranks each hold only their own part).  Errors go to E.
+static int walk_trace(Engine& E, const std::vector<Engine*>& ranks, Counterexample& x) {
+  std::vector<std::vector<uint64_t>> rev{x.words};
+  std::vector<uint32_t> rev_act{(uint32_t)(x.meta >> 56)};
+  uint64_t meta = x.meta, guard = 0;
   while ((meta & 0x0000FFFFFFFFFFFFull) != NO_PARENT && guard++ < 100000) {
-    uint64_t idx = meta & IDX_MASK;
-    uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
-    if (prank != E.rank || idx - E.store_base >= E.max_states && idx >= E.store_base) break;  // parent lives on another rank
+    const uint64_t idx = meta & IDX_MASK;
+    const uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
+    Engine* P = nullptr;
+    for (Engine* r : ranks)
+      if (r->rank == prank) P = r;
+    if (!P || (idx >= P->store_base && idx - P->store_base >= P->max_states)) break;
     std::vector<uint64_t> st(W);
-    if (int rc = read_range(E, idx, 1, st.data(), &meta)) return rc;
+    CK(cudaSetDevice(P->device));
+    if (int rc = read_range(*P, idx, 1, st.data(), &meta)) {
+      E.last_error = P->last_error;
+      return rc;
+    }
     rev.push_back(st);
     rev_act.push_back((uint32_t)(meta >> 56));
   }
-  trace.assign(rev.rbegin(), rev.rend());
-  actions.assign(rev_act.rbegin(), rev_act.rend());
+  x.trace.assign(rev.rbegin(), rev.rend());
+  x.actions.assign(rev_act.rbegin(), rev_act.rend());
   return KMC_OK;
 }
 
+// The run's violation from the violator ring at the end of level `level` (the level being expanded, 0 for the init
+// insert): the pick, its level and its trace on this rank.
 static int build_trace(Engine& E, const DevCounters& h, uint64_t level) {
   uint64_t n = std::min<uint64_t>(h.viol_count, VIOL_RING);
   if (n == 0) return KMC_OK;
   std::vector<uint64_t> ring(n * VIOL_ROW);
   CK(cudaMemcpy(ring.data(), E.viol_ring, ring.size() * 8, cudaMemcpyDeviceToHost));
-  const uint64_t* best = nullptr;
-  for (uint64_t i = 0; i < n; ++i) {
-    const uint64_t* r = ring.data() + i * VIOL_ROW;
-    if (!best) { best = r; continue; }
-    bool r_dead = r[W + 2] == ~0ull, b_dead = best[W + 2] == ~0ull;
-    if (r_dead != b_dead) { if (r_dead) best = r; continue; }
-    if (r[W + 1] < best[W + 1] || (r[W + 1] == best[W + 1] && r[W] < best[W])) best = r;
-  }
-  E.viol_words.assign(best, best + W);
-  E.viol_meta = best[W];
-  if (int rc = walk_trace(E, best, best[W], E.trace, E.trace_actions)) return rc;
-  bool dead = best[W + 2] == ~0ull;
-  E.viol.kind = dead ? KMC_RESULT_DEADLOCK : KMC_RESULT_INVARIANT;
-  E.viol.invariant = dead ? -1 : (int32_t)best[W + 2];
-  E.viol.level = dead ? level : level + 1;
-  E.viol.trace_len = E.trace.size();
-  E.viol.fingerprint = best[W + 1];
+  const uint64_t* best = pick(ring.data(), n, -1);
+  Counterexample x;
+  x.inv = best[W + 2] == ~0ull ? -1 : (int32_t)best[W + 2];
+  x.level = x.inv < 0 ? level : level + 1;
+  take_row(x, best);
+  if (int rc = walk_trace(E, {&E}, x)) return rc;
+  E.viol = std::move(x);
   return KMC_OK;
 }
 
 // Level end of a "continue" run: every pending invariant that a state of level `level` violates (`fresh`: the inv_new
 // words of the ranks, ORed) is reported -- its violators at that level (before it, it had none) and its pick from the
-// per-invariant ring by build_trace's rule (smallest fingerprint, then smallest parent word).  `walk`: walk the pick's
-// trace now (one rank; multi_run walks across the ranks).  Then those invariants stop being pending and the rings empty.
-// A level with more discarded violators than the stage holds makes the report incomplete.
+// per-invariant ring.  `walk`: walk the pick's trace now (one rank; multi_run walks across the ranks).  Then those
+// invariants stop being pending and the rings empty.  A level with more discarded violators than the stage holds
+// makes the report incomplete.
 static int collect_invariants(Engine& E, const DevCounters& h, uint64_t level, uint64_t fresh, bool walk) {
   fresh &= E.inv_pending;
   if (h.inv_staged > (uint64_t)VIOL_RING) E.inv_complete = false;
@@ -1958,24 +1975,16 @@ static int collect_invariants(Engine& E, const DevCounters& h, uint64_t level, u
   std::vector<uint64_t> ring(n * VIOL_ROW);
   if (n) CK(cudaMemcpy(ring.data(), inv_ring_of(E.viol_ring), ring.size() * 8, cudaMemcpyDeviceToHost));
   for (uint64_t b = fresh; b; b &= b - 1) {
-    InvReport r;
-    r.inv = __builtin_ctzll(b);
-    r.level = level;
-    r.first_count = h.inv_count[r.inv];
-    const uint64_t* best = nullptr;
-    for (uint64_t k = 0; k < n; ++k) {
-      const uint64_t* row = ring.data() + k * VIOL_ROW;
-      if (!((row[W + 2] >> r.inv) & 1)) continue;
-      if (!best || row[W + 1] < best[W + 1] || (row[W + 1] == best[W + 1] && row[W] < best[W])) best = row;
-    }
-    if (best) {
-      r.fp = best[W + 1];
-      r.meta = best[W];
-      r.words.assign(best, best + W);
+    Counterexample x;
+    x.inv = __builtin_ctzll(b);
+    x.level = level;
+    x.first_count = h.inv_count[x.inv];
+    if (const uint64_t* best = pick(ring.data(), n, x.inv)) {
+      take_row(x, best);
       if (walk)
-        if (int rc = walk_trace(E, best, best[W], r.trace, r.actions)) return rc;
+        if (int rc = walk_trace(E, {&E}, x)) return rc;
     }
-    E.inv_reports.push_back(std::move(r));
+    E.inv_reports.push_back(std::move(x));
   }
   E.inv_pending &= ~fresh;
   const unsigned long long w[5] = {E.inv_pending, 0, 0, 0, h.viol_count};   // inv_pending .. inv_viol_seen
@@ -2014,7 +2023,7 @@ static int end_level(Engine& E, uint64_t inv_bound, bool shard, DevCounters& h) 
     if (shard) E.stats.levels = E.stats.depth;
     else E.stats.queue = E.level_count;
   }
-  if (h.viol_count && E.viol.kind == KMC_RESULT_OK && (shard || !h.fail)) build_trace(E, h, level);
+  if (h.viol_count && E.viol.words.empty() && (shard || !h.fail)) build_trace(E, h, level);
   if (INV_REPORT && E.cont && (shard || !h.fail)) return collect_invariants(E, h, level + 1, h.inv_new, true);
   return KMC_OK;
 }
@@ -2242,24 +2251,34 @@ int kmcm_coverage(const kmcm_ctx* c, uint64_t* action_gen, uint64_t* action_dist
 int kmcm_violation(const kmcm_ctx* c, kmc_violation_t* out) {
   if (!c || !out) return KMC_E_BADARG;
   if (!E.ran && E.level == 0) return KMC_E_STATE;
-  *out = E.viol;
+  const Counterexample& x = E.viol;
+  memset(out, 0, sizeof(*out));
+  out->kind = x.words.empty() ? KMC_RESULT_OK : x.inv < 0 ? KMC_RESULT_DEADLOCK : KMC_RESULT_INVARIANT;
+  out->invariant = x.inv;
+  out->level = x.level;
+  out->trace_len = x.trace.size();
+  out->fingerprint = x.fp;
+  return KMC_OK;
+}
+
+static int trace_state(const Counterexample& x, uint32_t i, uint64_t* buf, size_t cap_words, uint32_t* action_id) {
+  if (i >= x.trace.size() || cap_words < (size_t)W) return KMC_E_BADARG;
+  memcpy(buf, x.trace[i].data(), W * 8);
+  if (action_id) *action_id = x.actions[i];
   return KMC_OK;
 }
 
 int kmcm_trace_state(const kmcm_ctx* c, uint32_t i, uint64_t* buf, size_t cap_words, uint32_t* action_id) {
   if (!c || !buf) return KMC_E_BADARG;
-  if (i >= E.trace.size() || cap_words < (size_t)W) return KMC_E_BADARG;
-  memcpy(buf, E.trace[i].data(), W * 8);
-  if (action_id) *action_id = E.trace_actions[i];
-  return KMC_OK;
+  return trace_state(E.viol, i, buf, cap_words, action_id);
 }
 
 // the offending state of this rank (before any cross-rank trace walk): packed words + parent/action word
 int kmcm_violation_record(const kmcm_ctx* c, uint64_t* words, size_t cap_words, uint64_t* parent_meta) {
   if (!c || !words || !parent_meta || cap_words < (size_t)W) return KMC_E_BADARG;
-  if (E.viol.kind == KMC_RESULT_OK || E.viol_words.size() != (size_t)W) return KMC_E_STATE;
-  memcpy(words, E.viol_words.data(), W * 8);
-  *parent_meta = E.viol_meta;
+  if (E.viol.words.empty()) return KMC_E_STATE;
+  memcpy(words, E.viol.words.data(), W * 8);
+  *parent_meta = E.viol.meta;
   return KMC_OK;
 }
 
@@ -2269,10 +2288,12 @@ static bool inv_reports_readable(const kmcm_ctx* c, int* rc) {
   *rc = !M::HAS_INVARIANT_MASK ? KMC_E_BADARG : (c->ranks.empty() && E.world > 1) || (!E.ran && E.level == 0) ? KMC_E_STATE : KMC_OK;
   return *rc == KMC_OK;
 }
-static std::vector<const InvReport*> inv_reports_sorted(const Engine& e) {
-  std::vector<const InvReport*> v;
-  for (const InvReport& r : e.inv_reports) v.push_back(&r);
-  std::sort(v.begin(), v.end(), [](const InvReport* a, const InvReport* b) { return a->level != b->level ? a->level < b->level : a->inv < b->inv; });
+static std::vector<const Counterexample*> inv_reports_sorted(const Engine& e) {
+  std::vector<const Counterexample*> v;
+  for (const Counterexample& r : e.inv_reports) v.push_back(&r);
+  std::sort(v.begin(), v.end(), [](const Counterexample* a, const Counterexample* b) {
+    return a->level != b->level ? a->level < b->level : a->inv < b->inv;
+  });
   return v;
 }
 
@@ -2281,7 +2302,7 @@ int kmcm_invariant_reports(const kmcm_ctx* c, kmc_invariant_report_t* out, size_
   int rc;
   if (!inv_reports_readable(c, &rc)) return rc;
   std::lock_guard<std::mutex> g(E.mu);
-  const std::vector<const InvReport*> v = inv_reports_sorted(E);
+  const std::vector<const Counterexample*> v = inv_reports_sorted(E);
   *n = v.size();
   *complete = E.inv_complete ? 1 : 0;
   for (size_t k = 0; k < v.size() && k < cap; ++k) {
@@ -2303,13 +2324,8 @@ int kmcm_invariant_trace_state(const kmcm_ctx* c, int32_t invariant, uint32_t i,
   int rc;
   if (!inv_reports_readable(c, &rc)) return rc;
   std::lock_guard<std::mutex> g(E.mu);
-  for (const InvReport& r : E.inv_reports) {
-    if (r.inv != invariant) continue;
-    if (i >= r.trace.size()) return KMC_E_BADARG;
-    memcpy(buf, r.trace[i].data(), W * 8);
-    if (action_id) *action_id = r.actions[i];
-    return KMC_OK;
-  }
+  for (const Counterexample& r : E.inv_reports)
+    if (r.inv == invariant) return trace_state(r, i, buf, cap_words, action_id);
   return KMC_E_BADARG;
 }
 
@@ -2615,7 +2631,7 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
     if (E.level_count) E.widths.push_back(E.level_count);
     E.stats.levels = E.stats.depth = E.widths.size();
   }
-  if (mine[2] && E.viol.kind == KMC_RESULT_OK) {
+  if (mine[2] && E.viol.words.empty()) {
     DevCounters h;
     if ((rc = read_counters(E, &h))) return rc;
     build_trace(E, h, E.level - 1);
@@ -2724,33 +2740,6 @@ static int multi_create(kmcm_ctx* c, const char* options_json, int gpus) {
   return KMC_OK;
 }
 
-// The trace of a violator found on some rank, following the parent links from store to store.
-static void walk_ranks(kmcm_ctx* c, const std::vector<uint64_t>& words, uint64_t meta, std::vector<std::vector<uint64_t>>& trace,
-                       std::vector<uint32_t>& actions) {
-  const size_t n = c->ranks.size();
-  std::vector<std::vector<uint64_t>> rev;
-  std::vector<uint32_t> rev_act;
-  rev.push_back(words);
-  rev_act.push_back((uint32_t)(meta >> 56));
-  uint64_t guard = 0;
-  while ((meta & 0x0000FFFFFFFFFFFFull) != NO_PARENT && guard++ < 100000) {
-    const uint64_t idx = meta & IDX_MASK;
-    const uint32_t prank = (uint32_t)((meta >> 40) & 0xFF);
-    if (prank >= n) break;
-    const Engine& P = c->ranks[prank]->e;
-    if (idx >= P.max_states) break;
-    std::vector<uint64_t> sw(W);
-    if (cudaSetDevice(P.device) != cudaSuccess ||
-        cudaMemcpy(sw.data(), P.store + idx * W, W * 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
-        cudaMemcpy(&meta, P.parent + idx, 8, cudaMemcpyDeviceToHost) != cudaSuccess)
-      break;
-    rev.push_back(sw);
-    rev_act.push_back((uint32_t)(meta >> 56));
-  }
-  trace.assign(rev.rbegin(), rev.rend());
-  actions.assign(rev_act.rbegin(), rev_act.rend());
-}
-
 struct RankOutcome {
   int rc = KMC_OK;
   std::vector<uint64_t> levels;
@@ -2850,61 +2839,39 @@ static int multi_run(kmcm_ctx* c) {
     for (size_t r = 0; r < n; ++r) st.queue += out[0].board[r * BOARD_WORDS + 1];
   }
   st.wall_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
-  // violation: deadlocks (they belong to the level being expanded) before invariant violations, then the smallest
-  // fingerprint, then the rank -- the single-GPU rule -- and the parent links are followed from store to store
-  memset(&A.viol, 0, sizeof(A.viol));
-  A.viol.invariant = -1;
-  A.trace.clear();
-  A.trace_actions.clear();
-  const Engine* best = nullptr;
-  for (size_t r = 0; r < n; ++r) {
-    const Engine& R = c->ranks[r]->e;
-    if (R.viol.kind == KMC_RESULT_OK) continue;
-    if (!best) { best = &R; continue; }
-    const bool rd = R.viol.kind == KMC_RESULT_DEADLOCK, bd = best->viol.kind == KMC_RESULT_DEADLOCK;
-    if (rd != bd) { if (rd) best = &R; continue; }
-    if (R.viol.fingerprint < best->viol.fingerprint) best = &R;
-  }
-  if (best && !rc) {
-    walk_ranks(c, best->viol_words, best->viol_meta, A.trace, A.trace_actions);
-    A.viol = best->viol;
-    A.viol.trace_len = A.trace.size();
-    A.viol_words = best->viol_words;
-    A.viol_meta = best->viol_meta;
-  }
-  // per-invariant report: every rank reported the same invariants at the same levels (they share the board); the
-  // violators are summed and the pick is the rule's pick among the ranks' picks
+  // The ranks' picks merged in violator order (reports: the earliest level first; the ranks' violators of an invariant
+  // at that level summed), then walked from store to store.  Every rank reports the same invariants at the same
+  // levels (they share the board).  No tie between ranks needs breaking: a violator's row is written on the rank that
+  // owns its fingerprint (owner_of(state_fp(s))), or on the rank that expands it, which for a deadlock is its owner
+  // too, so no two ranks hold candidates with the same fingerprint.
+  Counterexample viol;
   A.inv_reports.clear();
   A.inv_complete = true;
   std::fill(A.inv_count.begin(), A.inv_count.end(), 0);
+  std::vector<Engine*> ranks;
   for (size_t r = 0; r < n; ++r) {
-    const Engine& R = c->ranks[r]->e;
+    Engine& R = c->ranks[r]->e;
+    ranks.push_back(&R);
+    if (better(R.viol, viol)) viol = R.viol;
     A.inv_complete = A.inv_complete && R.inv_complete;
     for (size_t i = 0; i < A.inv_count.size(); ++i) A.inv_count[i] += R.inv_count[i];
-    for (const InvReport& x : R.inv_reports) {
-      InvReport* y = nullptr;
-      for (InvReport& a : A.inv_reports)
-        if (a.inv == x.inv) y = &a;
-      if (!y || x.level < y->level) {
-        if (!y) {
-          A.inv_reports.emplace_back();
-          y = &A.inv_reports.back();
-        }
+    for (const Counterexample& x : R.inv_reports) {
+      auto y = std::find_if(A.inv_reports.begin(), A.inv_reports.end(), [&](const Counterexample& a) { return a.inv == x.inv; });
+      if (y == A.inv_reports.end()) {
+        A.inv_reports.push_back(x);
+      } else if (x.level < y->level) {
         *y = x;
-        continue;
-      }
-      if (x.level > y->level) continue;
-      y->first_count += x.first_count;
-      if (!x.words.empty() && (y->words.empty() || x.fp < y->fp || (x.fp == y->fp && x.meta < y->meta))) {
-        y->fp = x.fp;
-        y->meta = x.meta;
-        y->words = x.words;
+      } else if (x.level == y->level) {
+        const uint64_t count = y->first_count + x.first_count;
+        if (better(x, *y)) *y = x;
+        y->first_count = count;
       }
     }
   }
-  if (!rc)
-    for (InvReport& a : A.inv_reports)
-      if (!a.words.empty()) walk_ranks(c, a.words, a.meta, a.trace, a.actions);
+  A.viol = rc ? Counterexample() : std::move(viol);
+  if (!rc && !A.viol.words.empty()) rc = walk_trace(A, ranks, A.viol);
+  for (Counterexample& x : A.inv_reports)
+    if (!rc && !x.words.empty()) rc = walk_trace(A, ranks, x);
   A.ran = true;
   return rc;
 }

@@ -1,9 +1,10 @@
-// Test harness (NOT a product path): a lowered model.h compiled for the host, so that the tests can run the header the
-// CUDA engine includes on a machine without a GPU.  tests/support/hostmodel.py builds one library per header text:
-//   g++ -O2 -std=c++17 -shared -fPIC -DKMC_MODEL_HEADER='"model.h"' host_model.cpp
+// Test harness (NOT a product path): a lowered model.h and its invariants.h compiled for the host, so that the tests can
+// run the headers the CUDA engine includes on a machine without a GPU.  tests/support/hostmodel.py builds one library
+// per header pair:
+//   g++ -O2 -std=c++17 -shared -fPIC -DKMC_MODEL_HEADER='"model.h"' -DKMC_INVARIANTS_HEADER='"invariants.h"' host_model.cpp
 // It holds
-//   hm_*     the model's facts and per-state calls: successors under either form of Next, invariants, constraints,
-//            initial states, canonical forms
+//   hm_*     the model's facts and per-state calls: successors under either form of Next, invariants (first violated and
+//            the mask of all violated), constraints, initial states, canonical forms
 //   hm_bfs   a level-ordered sequential BFS that stores its states as the engine does, with the run's statistics
 //   audit_*  the whole-store audit of a finished or stopped GPU run
 //   hs_*     a stand-in for one rank of the sharded engine (kafka_specification_b200/sharded.py's CPU tests)
@@ -17,6 +18,7 @@
 #include <unordered_set>
 #include <vector>
 #include KMC_MODEL_HEADER
+#include KMC_INVARIANTS_HEADER
 
 namespace M = kmc_model;
 using M::State;
@@ -132,6 +134,7 @@ int hm_successors(const uint64_t* state, int sites, uint64_t* out, int* actions,
   return (int)sink.out.size();
 }
 int hm_first_violated(const uint64_t* state) { return M::first_violated_invariant(load(state)); }
+uint64_t hm_mask(const uint64_t* state) { return M::violated_invariants(load(state)); }
 int hm_in_model(const uint64_t* state) { return M::in_model(load(state)) ? 1 : 0; }
 void hm_init_state(int i, uint64_t* out) { memcpy(out, M::INIT_STATES[i], sizeof(uint64_t) * W); }
 void hm_canonicalize(const uint64_t* states, uint64_t n, uint64_t* out) {
@@ -144,15 +147,21 @@ void hm_canonicalize(const uint64_t* states, uint64_t n, uint64_t* out) {
 
 // ================================================================================================ the BFS
 namespace {
-enum { T_GENERATED, T_DEADLOCKS, T_FAIL, T_COMPLETE, T_EXPANDED, T_MAX_FANOUT, T_FIRST_INV, T_FIRST_LEVEL, T_COUNT };
+enum { T_GENERATED, T_DEADLOCKS, T_FAIL, T_COMPLETE, T_EXPANDED, T_MAX_FANOUT, T_FIRST_INV, T_FIRST_LEVEL, T_MISMATCHES,
+       T_COUNT };
 // The last hm_bfs run, which the caller copies out with hm_bfs_array.
 struct Bfs {
   // generated (initial states included), deadlocks, fail code, complete, levels expanded, max fan-out,
-  // first violated invariant (~0: none) and its level
+  // first violated invariant (~0: none) and its level, checked states on which the mask and first_violated_invariant
+  // disagree
   std::vector<uint64_t> totals;
   std::vector<uint64_t> states, parents, widths;   // the store: W words per state, parent words, level widths
   std::vector<uint64_t> act_gen, site_gen;         // successors generated per action / per emit site
-  std::vector<uint64_t> inv_level, inv_count;      // per invariant: first violating level (0: never), violators
+  // per invariant, by first_violated_invariant: first violating level (0: never), violators
+  std::vector<uint64_t> inv_level, inv_count;
+  // per invariant, by the mask (what kmc_invariant_reports reports): first violating level (0: never), violators at
+  // that level, violators over the run, smallest set-identity fingerprint among that level's violators
+  std::vector<uint64_t> mask_level, mask_first_count, mask_count, mask_pick_fp;
 };
 Bfs g_bfs;
 }  // namespace
@@ -161,8 +170,9 @@ extern "C" {
 // Level-ordered sequential BFS (past violations, like -continue) that stores its states like the engine: in BFS order
 // (level k contiguous), the first member of an orbit found, parent words index | action << 56 (NO_PARENT for initial
 // states).  Successors come from expand() or, with sites, from the two-phase form, which also counts them per emit
-// site.  Every initial state, stored state and out-of-model successor is checked against the invariants.  Stops, as
-// incomplete, at the first level end that holds >= stop_at states (0: never) or at a layout trap.
+// site.  Every initial state, stored state and out-of-model successor (at its parent's level + 1, each time it is
+// generated) is checked against the invariants.  Stops, as incomplete, at the first level end that holds >= stop_at
+// states (0: never) or at a layout trap.
 void hm_bfs(int sites, uint64_t stop_at) {
   Bfs& B = g_bfs = Bfs();
   B.totals.assign(T_COUNT, 0);
@@ -172,10 +182,22 @@ void hm_bfs(int sites, uint64_t stop_at) {
   B.site_gen.assign(M::NUM_SITES, 0);
   B.inv_level.assign(M::NUM_INVARIANTS, 0);
   B.inv_count.assign(M::NUM_INVARIANTS, 0);
+  for (auto* v : {&B.mask_level, &B.mask_first_count, &B.mask_count}) v->assign(M::NUM_INVARIANTS, 0);
+  B.mask_pick_fp.assign(M::NUM_INVARIANTS, ~0ull);
   uint64_t* t = B.totals.data();
   StateSet seen;
   auto check = [&](const State& s, uint64_t level) {
+    const uint64_t m = M::violated_invariants(s);
     const int inv = M::first_violated_invariant(s);
+    if (m ? inv != __builtin_ctzll(m) : inv != -1) t[T_MISMATCHES]++;
+    for (uint64_t b = m; b; b &= b - 1) {
+      const int i = __builtin_ctzll(b);
+      B.mask_count[i]++;
+      if (!B.mask_level[i]) B.mask_level[i] = level;
+      if (B.mask_level[i] != level) continue;
+      B.mask_first_count[i]++;
+      B.mask_pick_fp[i] = std::min(B.mask_pick_fp[i], fingerprint(canon(s)));
+    }
     if (inv < 0) return;
     if (!B.inv_level[inv]) B.inv_level[inv] = level;
     B.inv_count[inv]++;
@@ -222,11 +244,12 @@ void hm_bfs(int sites, uint64_t stop_at) {
     first = end;
   }
 }
-// One array of the last run (0 totals, 1 states, 2 parents, 3 widths, 4 per action, 5 per site, 6 per invariant first
-// level, 7 per invariant violators): its length in *n and its words, valid until the next hm_bfs or hm_bfs_clear.
+// One array of the last run, in the order of Bfs's fields (hostmodel.py's BFS_ARRAYS): its length in *n and its words,
+// valid until the next hm_bfs or hm_bfs_clear.
 const uint64_t* hm_bfs_array(int which, uint64_t* n) {
-  std::vector<uint64_t>* v[] = {&g_bfs.totals,  &g_bfs.states,   &g_bfs.parents,   &g_bfs.widths,
-                                &g_bfs.act_gen, &g_bfs.site_gen, &g_bfs.inv_level, &g_bfs.inv_count};
+  std::vector<uint64_t>* v[] = {&g_bfs.totals,     &g_bfs.states,           &g_bfs.parents,    &g_bfs.widths,
+                                &g_bfs.act_gen,    &g_bfs.site_gen,         &g_bfs.inv_level,  &g_bfs.inv_count,
+                                &g_bfs.mask_level, &g_bfs.mask_first_count, &g_bfs.mask_count, &g_bfs.mask_pick_fp};
   *n = v[which]->size();
   return v[which]->data();
 }

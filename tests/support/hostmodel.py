@@ -1,7 +1,7 @@
 """Test support: a lowered model compiled for the host (host_model.cpp), its sequential BFS and per-state calls.
 
-One library per header text, built under build/hosttest/ on first use: a header lowered inside a test and the same
-header from build() share it."""
+One library per pair of header texts (model.h and invariants.h), built under build/hosttest/ on first use: headers
+lowered inside a test and the same headers from build() share it."""
 from __future__ import annotations
 
 import ctypes
@@ -34,6 +34,7 @@ SIGNATURES = {
     "hm_site_action": (_i32, [_i32]),
     "hm_successors": (_i32, [_vp, _i32, _vp, _vp, _i32]),
     "hm_first_violated": (_i32, [_vp]),
+    "hm_mask": (_u64, [_vp]),
     "hm_in_model": (_i32, [_vp]),
     "hm_init_state": (None, [_i32, _vp]),
     "hm_canonicalize": (None, [_vp, _u64, _vp]),
@@ -56,23 +57,25 @@ SIGNATURES = {
 }
 # hm_bfs_array's arrays, in its order
 BFS_ARRAYS = ("totals", "states", "parents", "widths", "action_generated", "site_generated", "invariant_first_level",
-              "invariant_violators")
+              "invariant_violators", "mask_first_level", "mask_violators_first_level", "mask_violators", "mask_pick")
 
 
-def _library_path(header_text: str) -> str:
-    """host_model.cpp compiled against `header_text`; written through pid-unique temporaries, so that test processes
-    building the same header at once never see a partial file."""
+def _library_path(header_text: str, invariants_text: str) -> str:
+    """host_model.cpp compiled against `header_text` and `invariants_text`; written through pid-unique temporaries, so
+    that test processes building the same headers at once never see a partial file."""
     with open(SOURCE) as f:
-        tag = hashlib.sha256((header_text + f.read()).encode()).hexdigest()[:16]
+        tag = hashlib.sha256((header_text + "\0" + invariants_text + "\0" + f.read()).encode()).hexdigest()[:16]
     so = os.path.join(BUILD, f"{tag}.so")
     if not os.path.exists(so):
         os.makedirs(BUILD, exist_ok=True)
-        hdr, tmp = os.path.join(BUILD, f"{tag}.h"), f".{os.getpid()}.tmp"
-        with open(hdr + tmp, "w") as f:
-            f.write(header_text)
-        os.replace(hdr + tmp, hdr)
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", f'-DKMC_MODEL_HEADER="{hdr}"', SOURCE,
-                               "-o", so + tmp])
+        tmp = f".{os.getpid()}.tmp"
+        hdr, inv = os.path.join(BUILD, f"{tag}.h"), os.path.join(BUILD, f"{tag}.inv.h")
+        for path, text in ((hdr, header_text), (inv, invariants_text)):
+            with open(path + tmp, "w") as f:
+                f.write(text)
+            os.replace(path + tmp, path)
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", f'-DKMC_MODEL_HEADER="{hdr}"',
+                               f'-DKMC_INVARIANTS_HEADER="{inv}"', SOURCE, "-o", so + tmp])
         os.replace(so + tmp, so)
     return so
 
@@ -87,11 +90,11 @@ def _load(so: str) -> ctypes.CDLL:
 
 
 class HostModel:
-    """host_model.cpp compiled against one model header."""
+    """host_model.cpp compiled against one model's model.h and invariants.h."""
 
-    def __init__(self, name: str, header_text: str):
+    def __init__(self, name: str, header_text: str, invariants_text: str):
         self.name = name
-        self.lib = lib = _load(_library_path(header_text))
+        self.lib = lib = _load(_library_path(header_text, invariants_text))
         self.words = lib.hm_words()
         self.state_bits = lib.hm_state_bits()
         self.all_ones_possible = bool(lib.hm_all_ones_possible())
@@ -106,14 +109,14 @@ class HostModel:
 
     @classmethod
     def from_lowered(cls, model: LoweredModel):
-        return cls(model.name, model.header)
+        return cls(model.name, model.header, model.invariants_header)
 
     @classmethod
     def for_built_model(cls, name: str):
-        """build/models/<name>/model.h, the header libkmc_<name>.so was compiled from."""
+        """build/models/<name>/model.h and invariants.h, the headers libkmc_<name>.so was compiled from."""
         d = os.path.join(ROOT, "build", "models", name)
-        with open(os.path.join(d, "model.h")) as f:
-            h = cls(name, f.read())
+        with open(os.path.join(d, "model.h")) as f, open(os.path.join(d, "invariants.h")) as g:
+            h = cls(name, f.read(), g.read())
         with open(os.path.join(d, "model.json")) as f:
             digest = json.load(f)["digest"]
         if h.digest != digest:
@@ -140,6 +143,10 @@ class HostModel:
     def first_violated(self, state) -> int:
         """Index of the first violated invariant, or -1."""
         return self.lib.hm_first_violated(self._state(state).ctypes.data)
+
+    def mask(self, state) -> int:
+        """Bit i set iff INVARIANT i is violated (violated_invariants)."""
+        return int(self.lib.hm_mask(self._state(state).ctypes.data))
 
     def in_model(self, state) -> bool:
         return bool(self.lib.hm_in_model(self._state(state).ctypes.data))
@@ -174,8 +181,22 @@ class HostModel:
         for key in BFS_ARRAYS[3:]:
             r[key] = [int(x) for x in r[key]]
         r.update(generated=t[0], deadlocks=t[1], fail=t[2], complete=bool(t[3]), n_expanded=t[4], max_fanout=t[5],
-                 first_invariant=None if t[6] == M64 else t[6], first_invariant_level=t[7])
+                 first_invariant=None if t[6] == M64 else t[6], first_invariant_level=t[7], mask_mismatches=t[8])
         return r
+
+    def invariant_report(self, invariants: list[str]) -> dict:
+        """What kmc_invariant_reports reports, from a full host BFS checked through the mask: {invariant name: {level,
+        violators_first_level, violators, fingerprint}} of the violated invariants, and the number of checked states
+        where the mask and first_violated_invariant disagree (key None)."""
+        assert len(invariants) == self.num_invariants
+        r = self.bfs()
+        if r["fail"]:
+            raise RuntimeError(f"{self.name}: layout trap (code {r['fail']}) during the host BFS")
+        out = {name: {"level": r["mask_first_level"][i], "violators_first_level": r["mask_violators_first_level"][i],
+                      "violators": r["mask_violators"][i], "fingerprint": r["mask_pick"][i]}
+               for i, name in enumerate(invariants) if r["mask_first_level"][i]}
+        out[None] = r["mask_mismatches"]
+        return out
 
 
 def run_host(model: LoweredModel, max_states: int = 0, dump: bool = False, items: bool = False) -> dict:

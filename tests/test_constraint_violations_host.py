@@ -56,7 +56,7 @@ def lowered(all_models, name):
 def audit_lib(all_models, name):
     from store_audit import AuditLib
     m = lowered(all_models, name)
-    return AuditLib(name, m.header)
+    return AuditLib(name, m.header, m.invariants_header)
 
 
 _ORACLE = {}

@@ -6,7 +6,6 @@ import random
 import pytest
 
 from conftest import REFERENCE, ROOT, needs_reference
-from hostinvariants import HostInvariants
 from hostmodel import HostModel, lower_model
 
 DIRS = [REFERENCE, os.path.join(ROOT, "models"), os.path.join(ROOT, "tests", "specs")]
@@ -33,7 +32,7 @@ def test_host_bfs_by_mask_gives_every_first_violation_level(name, goldens):
     violating level as the goldens record it (Oracle A's, and Oracle B's where it ran), constraint-discarded violators
     included; and on every checked state the mask agrees with first_violated_invariant."""
     m = _lower(name)
-    rep = HostInvariants.from_lowered(m).report()
+    rep = HostModel.from_lowered(m).invariant_report(m.invariants)
     assert rep.pop(None) == 0, "violated_invariants and first_violated_invariant disagree on a checked state"
     want = {i: l for i, l in goldens[name]["first_violation_level"].items() if l is not None}
     assert {i: r["level"] for i, r in rep.items()} == want
@@ -45,15 +44,16 @@ def test_host_bfs_by_mask_gives_every_first_violation_level(name, goldens):
 def test_two_invariants_at_one_level_and_a_discarded_only_violation(goldens):
     """minibound_mixed breaks NotOver and OneFull at level 3; asyncisr_bounded breaks VersionInBound only through
     successors its CONSTRAINT discards (the stored states never violate it)."""
-    rep = HostInvariants.from_lowered(_lower("minibound_mixed")).report()
+    mixed = _lower("minibound_mixed")
+    rep = HostModel.from_lowered(mixed).invariant_report(mixed.invariants)
     assert rep["NotOver"]["level"] == rep["OneFull"]["level"] == 3
     m = _lower("asyncisr_bounded")
-    rep = HostInvariants.from_lowered(m).report()
+    hm = HostModel.from_lowered(m)
+    rep = hm.invariant_report(m.invariants)
     assert rep["VersionInBound"]["level"] == goldens["asyncisr_bounded"]["first_violation_level"]["VersionInBound"]
-    r = HostModel.from_lowered(m).bfs()
-    hi = HostInvariants.from_lowered(m)
+    r = hm.bfs()
     bit = 1 << m.invariants.index("VersionInBound")
-    assert not any(hi.mask(s) & bit for s in r["states"])
+    assert not any(hm.mask(s) & bit for s in r["states"])
 
 
 # the walks of test_oracles_sampled.py, with Oracle A's verdict on every invariant of every state
@@ -70,7 +70,7 @@ def test_mask_on_random_walks_matches_oracle_a_and_first_violated(name, walks, s
     spec = _registry()[name]
     cfg_text = open(os.path.join(ROOT, spec["cfg"])).read()
     m = lower_model(spec["module"], DIRS, cfg_text, name=name)
-    hm, hi = HostModel.from_lowered(m), HostInvariants.from_lowered(m)
+    hm = HostModel.from_lowered(m)
     cfg = parse_cfg(cfg_text)
     it = tla_interp.Interp(load_root(spec["module"], DIRS), cfg)
     rng = random.Random(20260923 + len(name))
@@ -79,10 +79,10 @@ def test_mask_on_random_walks_matches_oracle_a_and_first_violated(name, walks, s
         cur = inits[rng.randrange(len(inits))].copy()
         for _ in range(steps):
             st = m.decode_state(cur)
-            mask = hi.mask(cur)
+            mask = hm.mask(cur)
             want = sum(1 << i for i, inv in enumerate(cfg.invariants) if not it.eval_named_predicate(inv, st))
             assert mask == want, (name, m.state_text(cur))
-            first = hi.first(cur)
+            first = hm.first_violated(cur)
             assert first == ((mask & -mask).bit_length() - 1 if mask else -1)
             rows, _ = hm.successors(cur)
             nxt = [r for r in rows if hm.in_model(r)]

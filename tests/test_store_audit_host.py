@@ -17,7 +17,7 @@ def _audit_lib(registry, name):
     spec = registry[name]
     m = lower_model(spec["module"], [REFERENCE, os.path.join(ROOT, "models")], open(os.path.join(ROOT, spec["cfg"])).read(),
                     name=name)
-    return AuditLib(name, m.header)
+    return AuditLib(name, m.header, m.invariants_header)
 
 
 @pytest.fixture(scope="module")

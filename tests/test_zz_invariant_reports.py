@@ -7,7 +7,7 @@ import sys
 import pytest
 
 from conftest import ROOT
-from hostinvariants import HostInvariants
+from hostmodel import HostModel
 from test_gpu_parity import _assert_trace_is_behaviour
 from test_zz_constraint_violations import OracleA
 
@@ -87,7 +87,7 @@ def test_every_violated_invariant_is_reported(name, goldens, all_models):
             assert (e["level"], e["fingerprint"], e["trace_len"]) == (v["level"], v["fingerprint"], v["trace_len"])
             assert [t["words"] for t in e["trace"]] == [t["words"] for t in r.trace]
         # the picks and counts against an independent host BFS of the lowered model, where the first level fits the ring
-        host = HostInvariants.for_built_model(name, ck.meta["invariants"]).report() if g["distinct"] < 3_000_000 else None
+        host = HostModel.for_built_model(name).invariant_report(ck.meta["invariants"]) if g["distinct"] < 3_000_000 else None
         for x in reps:
             if host is not None:
                 h = host[x["invariant"]]
