@@ -82,6 +82,11 @@ typedef struct {
   uint64_t complete;        /* 1 if the search ran to an empty queue                      */
   double gpu_ms_invariant;  /* sum over invariant-kernel launches (counted in launches_other) */
   uint64_t slot_bytes;      /* 8: 64-bit fingerprints (one-word states); 16: 128-bit keys (the state itself when it fits) */
+  uint64_t set_flushes;     /* "set_spill": times the table's keys moved to host memory                */
+  uint64_t set_host_keys;   /* "set_spill": keys in host memory (each distinct state's key at most once) */
+  uint64_t set_filtered;    /* "set_spill": appended states removed because their key was in host memory */
+  double gpu_ms_set_spill;  /* "set_spill": CUDA-event time of the flushes and filters (part of gpu_ms_total) */
+  uint64_t set_link_bytes;  /* "set_spill": key bytes the flushes (device to host) and filters (host to device) moved */
 } kmc_stats_t;
 
 typedef struct {
@@ -130,7 +135,12 @@ typedef struct {
  *   two; older levels move to host memory -- TLC's DiskStateQueue),
  * "checkpoint_dir":"d", "checkpoint_minutes":M (TLC -checkpoint: states + parent links + counters written at a level
  *   boundary at most every M minutes, 0 = every level; the per-site coverage counts are part of it),
- *   "recover":"d" (TLC -recover: continue from that checkpoint; the set is rebuilt from the stored states).
+ *   "recover":"d" (TLC -recover: continue from that checkpoint; the set is rebuilt from the stored states),
+ * "set_spill":false (one GPU only: when the fingerprint set's table would pass half its slots, its keys move to a host
+ *   memory array and the table starts empty, instead of the run ending in KMC_E_TABLE_FULL.  States appended since then
+ *   whose key is in host memory are removed before each move and at each level end, so the results are those of a run
+ *   with a table large enough.  With "spill" host memory bounds the run; about slot_bytes + 8 * words + 8 bytes per
+ *   state, and KMC_E_OOM when it runs out.  A set_spill context refuses "gpus" > 1, world > 1, the kmc_shard_* calls and kmc_fpset_*: KMC_E_BADARG).
  * Unknown keys are ignored.  */
 int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out);
 void kmc_destroy(kmc_ctx* ctx);

@@ -12,7 +12,7 @@ package tlc2.gpu;
 public final class GpuModelChecker {
     public static void main(String[] args) {
         String config = null, spec = null, modelLib = System.getProperty("kspec.model");
-        boolean noDeadlock = false, cont = false, spill = false;
+        boolean noDeadlock = false, cont = false, spill = false, setSpill = false;
         int gpus = 1, fpbits = 0;
         String metadir = null, recover = null;
         double checkpointMinutes = -1;
@@ -31,6 +31,7 @@ public final class GpuModelChecker {
                 case "-checkpoint": checkpointMinutes = Double.parseDouble(args[++i]); break;
                 case "-recover": recover = args[++i]; break;
                 case "-spill": spill = true; break;    // extension: old BFS levels move to host memory
+                case "-setspill": setSpill = true; break;    // extension: the set's keys move to host memory when its table fills
                 default: spec = args[i];
             }
         }
@@ -44,6 +45,7 @@ public final class GpuModelChecker {
         if (gpus > 1) opts.append(", \"gpus\": ").append(gpus);
         if (fpbits > 0) opts.append(", \"table_log2\": ").append(fpbits);
         if (spill) opts.append(", \"spill\": true");
+        if (setSpill) opts.append(", \"set_spill\": true");
         if (metadir != null) {
             opts.append(", \"checkpoint_dir\": \"").append(metadir).append("\"");
             opts.append(", \"checkpoint_minutes\": ").append(checkpointMinutes < 0 ? 30.0 : checkpointMinutes);

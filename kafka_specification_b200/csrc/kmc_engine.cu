@@ -35,6 +35,7 @@
 // There is no CPU fallback anywhere in this file: without a CUDA device kmc_create fails with
 // KMC_E_NO_GPU.
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -43,6 +44,7 @@
 #include <algorithm>
 #include <chrono>
 #include <mutex>
+#include <new>
 #include <thread>
 #include <string>
 #include <tuple>
@@ -181,6 +183,7 @@ struct DevCounters {
   unsigned long long inv_staged;         // discarded violators staged since the last level end
   unsigned long long inv_viol_seen;      // viol_count at the last level end (host-written)
   unsigned long long inv_count[64];      // violators per invariant over the run
+  unsigned long long set_count;          // set_spill: keys a flush range copied out, or states a filter piece kept
 };
 
 // Violating states are rare and terminal, so they go to a small ring: W state words, the
@@ -389,26 +392,32 @@ __device__ __forceinline__ int set_insert(void* table, uint64_t bucket_mask, con
   return set_insert_pre(table, bucket_mask, id, ld_bucket(table, bucket_of(id.fp, bucket_mask)), probes);
 }
 
-__device__ __forceinline__ int set_contains(const void* table, uint64_t bucket_mask, const Ident& id) {
+// returns the slot that holds the key (bucket * BUCKET_SLOTS + position), or -1 when it is absent
+__device__ __forceinline__ long long set_contains(const void* table, uint64_t bucket_mask, const Ident& id) {
   uint64_t b = bucket_of(id.fp, bucket_mask);
   for (int attempt = 0; attempt < 512; ++attempt) {
     Bucket bk = ld_bucket(table, b);
     bool any_empty = false;
+    const long long first = (long long)(b * BUCKET_SLOTS);
     if constexpr (KEY128) {
 #pragma unroll
       for (int k = 0; k < BUCKET_SLOTS; ++k) {
-        if (bk.v[k].x == id.key.lo && bk.v[k].y == id.key.hi) return 1;
+        if (bk.v[k].x == id.key.lo && bk.v[k].y == id.key.hi) return first + k;
         any_empty |= (bk.v[k].x & bk.v[k].y) == ~0ull;
       }
     } else {
       const uint64_t fp = id.fp;
-      if (bk.v[0].x == fp || bk.v[0].y == fp || bk.v[1].x == fp || bk.v[1].y == fp) return 1;
-      any_empty = bk.v[0].x == 0 || bk.v[0].y == 0 || bk.v[1].x == 0 || bk.v[1].y == 0;
+      const uint64_t v[4] = {bk.v[0].x, bk.v[0].y, bk.v[1].x, bk.v[1].y};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        if (v[k] == fp) return first + k;
+        any_empty |= v[k] == 0;
+      }
     }
-    if (any_empty) return 0;
+    if (any_empty) return -1;
     b = (b + 1) & bucket_mask;
   }
-  return 0;
+  return -1;
 }
 
 // Warp-collective insert of one candidate row per lane (invalid lanes pass valid = false):
@@ -1254,8 +1263,172 @@ __global__ void k_fpset_put(void* table, uint64_t bucket_mask, const uint64_t* f
       if (r > 0) atomicAdd(&ctr->store_tail, 1ull);
       seen[i] = r == 0;
     } else {
-      seen[i] = (uint8_t)set_contains(table, bucket_mask, id);
+      seen[i] = set_contains(table, bucket_mask, id) >= 0 ? 1 : 0;
     }
+  }
+}
+
+// ----------------------------------------------------------------------------------------
+// set_spill: the keys of the set move to host memory when the table fills (DESIGN.md section 3)
+// ----------------------------------------------------------------------------------------
+// An epoch is the time between two flushes.  k_set_flush copies the table's keys out (except those the last filter
+// found in host memory already) and the host empties the table.  The filter (k_set_mark, then k_set_compact) removes
+// from the states appended since the last filter those whose key is in host memory: they were found in an earlier epoch.
+static constexpr int KEY_WORDS = SLOT_BYTES / 8;
+static constexpr int SET_TILE = 256;          // states per tile of the filter's compaction
+
+// The identity a stored key stands for: the key alone gives the fingerprint that picks its bucket.
+__device__ __forceinline__ Ident key_ident(const uint64_t* k) {
+  Ident id;
+  if constexpr (!KEY128) {
+    id.fp = k[0];
+    id.key = Key128{0, 0};
+  } else if constexpr (W == 2 && !M::ALL_ONES_POSSIBLE) {
+    State s;                                   // the key is the packed (canonical) state itself
+    s.w[0] = k[0];
+    s.w[W - 1] = k[1];
+    id.fp = fingerprint(s);
+    id.key = Key128{k[0], k[1]};
+  } else {
+    id.fp = k[0];                              // the fingerprint is the key's low word
+    id.key = Key128{k[0], k[1]};
+  }
+  return id;
+}
+
+__device__ __forceinline__ bool marked(const unsigned* marks, long long slot) {
+  return slot >= 0 && ((marks[slot >> 5] >> (slot & 31)) & 1u);
+}
+
+// Slots [first, first + n) of the table: every key that is not marked goes to `out`, compacted with ballot/popc (the
+// order does not matter), counted in ctr->set_count.
+__global__ void __launch_bounds__(256) k_set_flush(const void* table, uint64_t first, uint64_t n, const unsigned* marks,
+                                                    uint64_t* out, DevCounters* ctr) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const unsigned lane = lane_id();
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ((n + 31) & ~31ull); i += stride) {
+    const uint64_t slot = first + i;
+    uint64_t k[KEY_WORDS];
+    bool take = false;
+    if (i < n) {
+      const uint64_t* src = static_cast<const uint64_t*>(table) + slot * KEY_WORDS;
+#pragma unroll
+      for (int w = 0; w < KEY_WORDS; ++w) k[w] = src[w];
+      const bool full = KEY128 ? (k[0] & k[KEY_WORDS - 1]) != ~0ull : k[0] != 0;
+      take = full && !marked(marks, (long long)slot);
+    }
+    const unsigned who = __ballot_sync(0xffffffffu, take);
+    if (!who) continue;
+    unsigned long long base = 0;
+    if ((int)lane == __ffs(who) - 1) base = atomicAdd(&ctr->set_count, (unsigned long long)__popc(who));
+    base = __shfl_sync(0xffffffffu, base, __ffs(who) - 1);
+    if (take) {
+      uint64_t* dst = out + (base + __popc(who & ((1u << lane) - 1))) * KEY_WORDS;
+#pragma unroll
+      for (int w = 0; w < KEY_WORDS; ++w) dst[w] = k[w];
+    }
+  }
+}
+
+// n host keys (one chunk of the stream through HBM): each one found in the table marks its slot.
+__global__ void __launch_bounds__(256) k_set_mark(const void* table, uint64_t bucket_mask, const uint64_t* keys, uint64_t n,
+                                                   unsigned* marks) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long slot = set_contains(table, bucket_mask, key_ident(keys + i * KEY_WORDS));
+    if (slot >= 0) atomicOr(marks + (slot >> 5), 1u << (slot & 31));
+  }
+}
+
+// The filter's verdict on the states [first, first + n) of the store: a state is removed when the slot of its identity
+// (state_ident: the orbit representative under SYMMETRY) is marked.  keep[j] = 1 for a survivor, tile_count[t] = the
+// survivors of tile t, and the removed states leave the per-action distinct counts (their parent words' actions).
+__global__ void __launch_bounds__(SET_TILE) k_set_compact(Params p, uint64_t first, uint64_t n, const unsigned* marks,
+                                                           uint8_t* keep, unsigned long long* tile_count) {
+  __shared__ unsigned long long removed[M::NUM_ACTIONS > 0 ? M::NUM_ACTIONS : 1];
+  for (unsigned a = threadIdx.x; a < (unsigned)M::NUM_ACTIONS; a += SET_TILE) removed[a] = 0;
+  __syncthreads();
+  for (uint64_t t = blockIdx.x; t * SET_TILE < n; t += gridDim.x) {
+    const uint64_t j = t * SET_TILE + threadIdx.x;
+    bool kept = false;
+    if (j < n) {
+      const uint64_t g = (first + j) & p.store_mask;
+      State s;
+#pragma unroll
+      for (int k = 0; k < W; ++k) s.w[k] = p.store[g * W + k];
+      kept = !marked(marks, set_contains(p.table, p.bucket_mask, state_ident(s)));
+      keep[j] = kept ? 1 : 0;
+      if (!kept) {
+        const uint64_t meta = p.parent[g];
+        const unsigned act = ((meta & 0x0000FFFFFFFFFFFFull) == NO_PARENT) ? ~0u : (unsigned)(meta >> 56);
+        if (act < (unsigned)M::NUM_ACTIONS) atomicAdd(&removed[act], 1ull);
+      }
+    }
+    const int c = __syncthreads_count(kept);
+    if (threadIdx.x == 0) tile_count[t] = (unsigned long long)c;
+  }
+  __syncthreads();
+  for (unsigned a = threadIdx.x; a < (unsigned)M::NUM_ACTIONS; a += SET_TILE)
+    if (removed[a]) atomicAdd(&p.ctr->action_distinct[a], 0ull - removed[a]);
+}
+
+// One CTA: tile_count[0, n) -> exclusive prefix sums in place; ctr->set_count = the total.
+__global__ void __launch_bounds__(1024) k_set_scan(unsigned long long* tile_count, uint64_t n, DevCounters* ctr) {
+  __shared__ unsigned long long warp_sum[32];
+  __shared__ unsigned long long carry;
+  const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (uint64_t base = 0; base < n; base += 1024) {
+    const uint64_t i = base + threadIdx.x;
+    const unsigned long long v = i < n ? tile_count[i] : 0;
+    unsigned long long x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+      if ((int)lane >= o) x += y;
+    }
+    if (lane == 31) warp_sum[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      unsigned long long s = warp_sum[lane];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, s, o);
+        if ((int)lane >= o) s += y;
+      }
+      warp_sum[lane] = s;
+    }
+    __syncthreads();
+    if (i < n) tile_count[i] = carry + (warp ? warp_sum[warp - 1] : 0) + x - v;
+    __syncthreads();
+    if (threadIdx.x == 0) carry += warp_sum[31];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) ctr->set_count = carry;
+}
+
+// The survivors of [first, first + n), in their order, to out_states / out_parents at their tiles' offsets.
+__global__ void __launch_bounds__(SET_TILE) k_set_scatter(Params p, uint64_t first, uint64_t n, const uint8_t* keep,
+                                                           const unsigned long long* tile_off, uint64_t* out_states,
+                                                           uint64_t* out_parents) {
+  __shared__ unsigned warp_kept[SET_TILE / 32];
+  const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
+  for (uint64_t t = blockIdx.x; t * SET_TILE < n; t += gridDim.x) {
+    const uint64_t j = t * SET_TILE + threadIdx.x;
+    const bool kept = j < n && keep[j];
+    const unsigned who = __ballot_sync(0xffffffffu, kept);
+    if (lane == 0) warp_kept[warp] = __popc(who);
+    __syncthreads();
+    if (kept) {
+      uint64_t o = tile_off[t] + __popc(who & ((1u << lane) - 1));
+      for (unsigned w = 0; w < warp; ++w) o += warp_kept[w];
+      const uint64_t g = (first + j) & p.store_mask;
+#pragma unroll
+      for (int k = 0; k < W; ++k) out_states[o * W + k] = p.store[g * W + k];
+      out_parents[o] = p.parent[g];
+    }
+    __syncthreads();
   }
 }
 
@@ -1263,7 +1436,7 @@ __global__ void k_fpset_put(void* table, uint64_t bucket_mask, const uint64_t* f
 // host side
 // ----------------------------------------------------------------------------------------
 struct LaunchRec {
-  int kind;  // 0 expand, 1 insert, 2 other
+  int kind;  // 0 expand, 1 insert, 2 other, 3 set_spill's flushes and filters
   cudaEvent_t a, b;
 };
 
@@ -1299,6 +1472,21 @@ struct Engine {
   std::string checkpoint_dir, recover_dir;
   double checkpoint_minutes = 0;    // 0: a checkpoint after every level (when checkpoint_dir is set)
   std::chrono::steady_clock::time_point last_checkpoint;
+  // set_spill (single rank): the keys of the set move to host memory whenever the table would pass set_limit(); the
+  // filter's marks (a bit per table slot) and its staging and compaction space live at the end and the start of `cand`
+  bool set_spill = false;
+  // the keys in host memory, KEY_WORDS words each as the table stores them: one block of exactly its size per flushed
+  // slot range, so that the array grows without the copies (and the transient double size) of a growing vector
+  std::vector<std::vector<uint64_t>> host_keys;
+  uint64_t set_host_keys = 0;           // keys in host_keys
+  uint64_t set_keys = 0;                // keys inserted into the table since the last flush
+  uint64_t set_tail = 0;                // the store tail set_keys was last brought up to date with
+  uint64_t set_from = 0;                // the first state the filter has not checked against host_keys
+  uint64_t set_flushes = 0, set_filtered = 0, set_link_bytes = 0;
+  uint64_t set_stage_keys = 0;          // keys per pinned staging buffer of the filter's key stream
+  uint64_t* set_pinned[2] = {};
+  cudaStream_t set_copy_stream = nullptr;
+  cudaEvent_t set_copied[2] = {}, set_probed[2] = {};
 
   void* table = nullptr;
   uint64_t table_slots = 0;             // slots of SLOT_BYTES each
@@ -1550,6 +1738,183 @@ static int engine_alloc(Engine& E) {
   return KMC_OK;
 }
 
+// ---- set_spill: host side ----------------------------------------------------------------------------------------
+// The table takes keys up to half its slots per epoch (the probe sequence stays short); then its keys move to host
+// memory.  cand (unused by the single-rank fused path) holds the marks at its end and the filter's and the flush's
+// working space before them.
+static uint64_t set_limit(const Engine& E) { return E.table_slots / 2; }
+static uint64_t set_mark_words(const Engine& E) { return (E.table_slots + 63) / 64; }
+static uint64_t set_scratch_words(const Engine& E) { return E.region_rows * E.world * ROW - set_mark_words(E); }
+static unsigned* set_marks(const Engine& E) { return reinterpret_cast<unsigned*>(E.cand + set_scratch_words(E)); }
+// states per compaction piece: W + 1 words of survivors, a keep byte and a tile counter each
+static uint64_t set_piece(const Engine& E) { return set_scratch_words(E) / (ROW + 1) / SET_TILE * SET_TILE; }
+
+static int set_alloc(Engine& E) {
+  const uint64_t limit = set_limit(E);
+  if (limit < (uint64_t)M::MAX_FANOUT) {
+    E.last_error = "set_spill: half the table's slots must hold one state's successors (raise table_log2)";
+    return KMC_E_BADARG;
+  }
+  if (E.region_rows * E.world * ROW <= set_mark_words(E) || set_piece(E) == 0) {
+    E.last_error = "set_spill: the candidate buffer cannot hold the filter's marks and working space (raise cand_bytes)";
+    return KMC_E_BADARG;
+  }
+  E.set_stage_keys = std::min<uint64_t>(1 << 20, set_scratch_words(E) / (2 * KEY_WORDS));
+  for (int b = 0; b < 2; ++b) {
+    CK(cudaHostAlloc(&E.set_pinned[b], E.set_stage_keys * SLOT_BYTES, cudaHostAllocDefault));
+    CK(cudaEventCreateWithFlags(&E.set_copied[b], cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&E.set_probed[b], cudaEventDisableTiming));
+  }
+  CK(cudaStreamCreateWithFlags(&E.set_copy_stream, cudaStreamNonBlocking));
+  return KMC_OK;
+}
+
+static uint64_t ring_run(const Engine& E, uint64_t g, uint64_t end, uint64_t* slot);
+
+// The store tail and the fail flag (one copy: the counters from store_tail to fail are contiguous).
+static int read_tail(Engine& E, uint64_t* tail, uint64_t* fail) {
+  constexpr size_t first = offsetof(DevCounters, store_tail), end = offsetof(DevCounters, fail) + 8;
+  unsigned long long w[(end - first) / 8];
+  CK(cudaMemcpyAsync(w, &E.ctr->store_tail, end - first, cudaMemcpyDeviceToHost, E.stream));
+  CK(cudaStreamSynchronize(E.stream));
+  *tail = w[0];
+  *fail = w[(end - first) / 8 - 1];
+  return KMC_OK;
+}
+
+// Every key of the table that the last filter did not find in host memory is appended to host_keys, in slot ranges that
+// fit the scratch space; then the table and the marks are emptied and a new epoch begins.  Host memory running out is
+// KMC_E_OOM.
+static int set_flush(Engine& E) {
+  TimedLaunch t(E, 3);
+  const uint64_t range = set_scratch_words(E) / KEY_WORDS;
+  for (uint64_t s0 = 0; s0 < E.table_slots; s0 += range) {
+    const uint64_t n = std::min(range, E.table_slots - s0);
+    CK(cudaMemsetAsync(&E.ctr->set_count, 0, sizeof(unsigned long long), E.stream));
+    k_set_flush<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, s0, n, set_marks(E), E.cand, E.ctr);
+    CK(cudaGetLastError());
+    unsigned long long k = 0;
+    CK(cudaMemcpyAsync(&k, &E.ctr->set_count, sizeof(k), cudaMemcpyDeviceToHost, E.stream));
+    CK(cudaStreamSynchronize(E.stream));
+    if (k == 0) continue;
+    try {
+      E.host_keys.emplace_back(k * KEY_WORDS);
+    } catch (const std::bad_alloc&) {
+      E.last_error = "set_spill: host memory for the fingerprint set's keys is exhausted";
+      return KMC_E_OOM;
+    }
+    CK(cudaMemcpy(E.host_keys.back().data(), E.cand, k * SLOT_BYTES, cudaMemcpyDeviceToHost));
+    E.set_host_keys += k;
+    E.set_link_bytes += k * SLOT_BYTES;
+  }
+  CK(cudaMemsetAsync(E.table, KEY128 ? 0xFF : 0, E.table_slots * SLOT_BYTES, E.stream));
+  CK(cudaMemsetAsync(set_marks(E), 0, set_mark_words(E) * 8, E.stream));
+  E.set_keys = 0;
+  E.set_from = E.set_tail;
+  E.set_flushes++;
+  return KMC_OK;
+}
+
+// Marks the slot of every table key that is in host memory: the host keys stream through two pinned buffers into two
+// staging areas of the scratch space, the copy of one chunk (on its own stream) overlapping the probes of the previous.
+static int set_mark(Engine& E) {
+  const uint64_t S = E.set_stage_keys;
+  uint64_t* stage[2] = {E.cand, E.cand + S * KEY_WORDS};
+  const uint64_t bucket_mask = E.table_slots / BUCKET_SLOTS - 1;
+  // the staging areas are free once the work already on the engine stream (which may use the scratch space) is done
+  for (int b = 0; b < 2; ++b) CK(cudaEventRecord(E.set_probed[b], E.stream));
+  uint64_t k = 0;
+  for (const std::vector<uint64_t>& block : E.host_keys) {
+    const uint64_t nkeys = block.size() / KEY_WORDS;
+    for (uint64_t i = 0; i < nkeys; i += S, ++k) {
+      const int b = (int)(k & 1);
+      const uint64_t n = std::min(S, nkeys - i);
+      CK(cudaEventSynchronize(E.set_probed[b]));          // the probes of chunk k - 2 are done with buffer b
+      memcpy(E.set_pinned[b], block.data() + i * KEY_WORDS, n * SLOT_BYTES);
+      CK(cudaStreamWaitEvent(E.set_copy_stream, E.set_probed[b], 0));
+      CK(cudaMemcpyAsync(stage[b], E.set_pinned[b], n * SLOT_BYTES, cudaMemcpyHostToDevice, E.set_copy_stream));
+      CK(cudaEventRecord(E.set_copied[b], E.set_copy_stream));
+      CK(cudaStreamWaitEvent(E.stream, E.set_copied[b], 0));
+      k_set_mark<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, bucket_mask, stage[b], n, set_marks(E));
+      CK(cudaGetLastError());
+      CK(cudaEventRecord(E.set_probed[b], E.stream));
+    }
+  }
+  E.set_link_bytes += E.set_host_keys * SLOT_BYTES;
+  return KMC_OK;
+}
+
+// The filter: the states appended since the last one whose key is in host memory were found in an earlier epoch.  They
+// are removed, and the survivors are compacted in place, in their order, piece by piece (a piece's survivors go to the
+// scratch space, then back to the store behind the previous pieces' survivors): nothing points at the level being
+// built until it is expanded.  store_tail, set_filtered and the per-action distinct counts follow.
+// After a failure the filter does nothing and end_level reports the error: once the store is full, the inserts still
+// count store_tail up but write no rows, so [set_from, tail) would reach past the store (or, in a ring, onto the
+// frontier being expanded).
+static int set_filter(Engine& E) {
+  if (E.set_host_keys == 0) return KMC_OK;            // nothing flushed yet: every appended state is new
+  uint64_t tail, fail;
+  int rc = read_tail(E, &tail, &fail);
+  if (rc || fail) return rc;
+  E.set_keys += tail - E.set_tail;
+  E.set_tail = tail;
+  if (tail == E.set_from) return KMC_OK;
+  TimedLaunch t(E, 3);
+  if ((rc = set_mark(E))) return rc;
+  const uint64_t P = set_piece(E);
+  uint64_t* out_states = E.cand;
+  uint64_t* out_parents = out_states + P * W;
+  uint8_t* keep = reinterpret_cast<uint8_t*>(out_parents + P);
+  unsigned long long* tiles = reinterpret_cast<unsigned long long*>(keep + P);
+  const Params p = E.params();
+  uint64_t cursor = E.set_from;
+  for (uint64_t g = E.set_from; g < tail; g += P) {
+    const uint64_t n = std::min(P, tail - g);
+    const int grid = grid_for(E, n, SET_TILE, 8);
+    k_set_compact<<<grid, SET_TILE, 0, E.stream>>>(p, g, n, set_marks(E), keep, tiles);
+    k_set_scan<<<1, 1024, 0, E.stream>>>(tiles, (n + SET_TILE - 1) / SET_TILE, E.ctr);
+    k_set_scatter<<<grid, SET_TILE, 0, E.stream>>>(p, g, n, keep, tiles, out_states, out_parents);
+    CK(cudaGetLastError());
+    unsigned long long kept = 0;
+    CK(cudaMemcpyAsync(&kept, &E.ctr->set_count, sizeof(kept), cudaMemcpyDeviceToHost, E.stream));
+    CK(cudaStreamSynchronize(E.stream));
+    for (uint64_t c = cursor, slot, m; c < cursor + kept; c += m) {
+      m = ring_run(E, c, cursor + kept, &slot);
+      CK(cudaMemcpyAsync(E.store + slot * W, out_states + (c - cursor) * W, m * W * 8, cudaMemcpyDeviceToDevice, E.stream));
+      CK(cudaMemcpyAsync(E.parent + slot, out_parents + (c - cursor), m * 8, cudaMemcpyDeviceToDevice, E.stream));
+    }
+    cursor += kept;
+  }
+  const unsigned long long new_tail = cursor;
+  CK(cudaMemcpyAsync(&E.ctr->store_tail, &new_tail, sizeof(new_tail), cudaMemcpyHostToDevice, E.stream));
+  CK(cudaStreamSynchronize(E.stream));
+  E.set_filtered += tail - cursor;
+  E.set_from = E.set_tail = cursor;
+  return KMC_OK;
+}
+
+// At a chunk boundary (one counter read): the table's keys of this epoch are brought up to date; when the room left
+// below set_limit() would cut the chunk below a quarter of the limit's worth of states, the epoch ends (filter, then
+// flush).  The chunk then gets at most room / MAX_FANOUT states -- MAX_FANOUT is a true bound on a state's successors,
+// unlike fanout_bound, an assumed average -- so its successors, and so its inserts, fit the room whatever the states;
+// Params::region_rows (the KMC_E_CAND_FULL check of the expand kernel) is capped to the room as well.  After a failure
+// the chunk is left as it is: the run ends at the level end with that error.
+static int set_room(Engine& E, uint64_t* count, uint64_t* bound) {
+  uint64_t tail, fail;
+  int rc = read_tail(E, &tail, &fail);
+  if (rc || fail) return rc;
+  E.set_keys += tail - E.set_tail;
+  E.set_tail = tail;
+  const uint64_t limit = set_limit(E), F = (uint64_t)M::MAX_FANOUT;
+  auto room = [&] { return E.set_keys < limit ? limit - E.set_keys : 0; };
+  if (room() / F < std::min<uint64_t>(*count, std::max<uint64_t>(1, limit / F / 4))) {
+    if ((rc = set_filter(E)) || (rc = set_flush(E))) return rc;
+  }
+  *count = std::min(*count, room() / F);
+  *bound = std::min(E.region_rows, room());
+  return KMC_OK;
+}
+
 static uint64_t all_invariants() { return M::NUM_INVARIANTS >= 64 ? ~0ull : (1ull << M::NUM_INVARIANTS) - 1; }
 
 // The per-invariant report starts afresh (every invariant pending) and, under "continue", the recorder is switched on.
@@ -1578,6 +1943,10 @@ static int engine_reset(Engine& E) {
   E.store_base = 0;
   E.host_store.clear();
   E.host_parent.clear();
+  E.host_keys.clear();
+  E.set_host_keys = 0;
+  E.set_keys = E.set_tail = E.set_from = E.set_flushes = E.set_filtered = E.set_link_bytes = 0;
+  if (E.set_spill) CK(cudaMemsetAsync(set_marks(E), 0, set_mark_words(E) * 8, E.stream));
   {
     std::lock_guard<std::mutex> g(E.mu);
     std::fill(E.site_generated.begin(), E.site_generated.end(), 0);
@@ -1600,6 +1969,10 @@ static void publish(Engine& E, const DevCounters& h, bool clamp) {
   st.table_slots = E.table_slots;
   st.slot_bytes = SLOT_BYTES;
   st.max_states = E.max_states;
+  st.set_flushes = E.set_flushes;
+  st.set_host_keys = E.set_host_keys;
+  st.set_filtered = E.set_filtered;
+  st.set_link_bytes = E.set_link_bytes;
   E.site_generated.assign(h.site_generated, h.site_generated + M::NUM_SITES);
   E.action_distinct.assign(h.action_distinct, h.action_distinct + M::NUM_ACTIONS);
   E.inv_count.assign(h.inv_count, h.inv_count + 64);
@@ -1674,11 +2047,12 @@ static int launch_invariants(Engine& E, uint64_t first, uint64_t count_bound) {
 }
 
 // fused (kmc_run, one rank): the kernel inserts the successors itself; otherwise they go to the candidate buffer
-// (or the owners' inboxes) for k_insert / k_insert_inbox
-static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false, bool fused = false) {
+// (or the owners' inboxes) for k_insert / k_insert_inbox.  cand_bound (set_spill): a smaller bound on the chunk's successors.
+static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false, bool fused = false, uint64_t cand_bound = 0) {
   Params p = E.params();
   p.p2p = p2p ? 1 : 0;
   p.fused = fused ? 1 : 0;
+  if (cand_bound) p.region_rows = cand_bound;
   if (count == 0) return KMC_OK;
   TimedLaunch t(E, 0);
   // small levels: smaller tiles so that every SM still gets one (a tile is a multiple of 32 states)
@@ -1872,15 +2246,22 @@ static int read_checkpoint(Engine& E, DevCounters* h) {
   if (rc) return rc;
   // the counters in one copy, before the rebuild: k_rebuild sets `fail` when the set overflows
   CK(cudaMemcpyAsync(E.ctr, h, sizeof(*h), cudaMemcpyHostToDevice, E.stream));
-  // rebuild the set: every stored state is inserted once, in batches through the candidate buffer
+  // rebuild the set: every stored state is inserted once, in batches through the candidate buffer.  With set_spill
+  // the batches stay clear of the marks, and the table is flushed whenever a batch would pass set_limit() (the states
+  // are distinct: no filter is needed)
   Params p = E.params();
-  const uint64_t batch = E.region_rows * ROW / W;
+  uint64_t batch = E.region_rows * ROW / W;
+  if (E.set_spill) batch = std::min(set_scratch_words(E) / W, set_limit(E));
   for (uint64_t g = 0; g < tail; g += batch) {
     const uint64_t n = std::min<uint64_t>(batch, tail - g);
+    if (E.set_spill && E.set_keys + n > set_limit(E))
+      if (int rc = set_flush(E)) return rc;
     CK(cudaMemcpyAsync(E.cand, st.data() + g * W, n * W * 8, cudaMemcpyHostToDevice, E.stream));
     k_rebuild<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(p, E.cand, n);
     CK(cudaStreamSynchronize(E.stream));
+    E.set_keys += n;
   }
+  E.set_tail = E.set_from = tail;
   DevCounters now;
   if ((rc = read_counters(E, &now))) return rc;
   if ((rc = fail_to_error(now.fail))) return rc;
@@ -1993,13 +2374,14 @@ static int collect_invariants(Engine& E, const DevCounters& h, uint64_t level, u
 }
 
 static void accumulate_timing(Engine& E, kmc_stats_t& st) {
-  st.gpu_ms_expand = st.gpu_ms_insert = st.gpu_ms_invariant = 0;
+  st.gpu_ms_expand = st.gpu_ms_insert = st.gpu_ms_invariant = st.gpu_ms_set_spill = 0;
   st.launches_expand = st.launches_insert = st.launches_other = 0;
   for (const LaunchRec& r : E.launches) {
     float ms = 0;
     cudaEventElapsedTime(&ms, r.a, r.b);
     if (r.kind == 0) { st.gpu_ms_expand += ms; st.launches_expand++; }
     else if (r.kind == 1) { st.gpu_ms_insert += ms; st.launches_insert++; }
+    else if (r.kind == 3) st.gpu_ms_set_spill += ms;
     else { st.gpu_ms_invariant += ms; st.launches_other++; }
   }
 }
@@ -2058,11 +2440,14 @@ static int engine_run(Engine& E) {
     const uint64_t level_end = E.level_first + E.level_count;
     for (uint64_t off = E.level_first, slot, cnt; off < level_end; off += cnt) {
       cnt = std::min<uint64_t>(E.chunk_states, ring_run(E, off, level_end, &slot));   // a chunk never crosses the wrap
+      uint64_t bound = 0;
+      if (E.set_spill && (rc = set_room(E, &cnt, &bound))) return rc;
       // one launch per chunk: the expand kernel inserts its successors itself (Params::fused); the candidate
       // counter only bounds the chunk's successors
       if ((rc = reset_cand(E))) return rc;
-      if ((rc = launch_expand(E, off, cnt, false, true))) return rc;
+      if ((rc = launch_expand(E, off, cnt, false, true, bound))) return rc;
     }
+    if (E.set_spill && (rc = set_filter(E))) return rc;         // before k_invariants sees the level
     if ((rc = end_level(E, E.level_count * 2, false, h))) return rc;
     err = fail_to_error(h.fail);
     if (!err && h.viol_count && !E.cont) {
@@ -2126,6 +2511,7 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
   if (json_bool(options_json, "timing", &b)) E.timing = b;
   if (json_num(options_json, "stop_after_states", &d)) E.stop_after_states = (uint64_t)d;
   if (json_bool(options_json, "spill", &b)) E.spill = b;
+  if (json_bool(options_json, "set_spill", &b)) E.set_spill = b;
   json_str(options_json, "checkpoint_dir", &E.checkpoint_dir);
   json_str(options_json, "recover", &E.recover_dir);
   if (json_num(options_json, "checkpoint_minutes", &d)) E.checkpoint_minutes = d;
@@ -2140,12 +2526,20 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
     delete c;
     return KMC_E_BADARG;
   }
-  if (json_num(options_json, "gpus", &d) && d > 1) {
+  const bool gpus = json_num(options_json, "gpus", &d) && d > 1;
+  if (E.set_spill && (gpus || E.world > 1)) {
+    // each rank's set would need the keys of the others' host memory too
+    E.last_error = "set_spill runs on one GPU (no \"gpus\" > 1, no world > 1)";
+    *out = c;
+    return KMC_E_BADARG;
+  }
+  if (gpus) {
     *out = c;
     return multi_create(c, options_json, (int)d);
   }
   int rc = engine_alloc(E);
   *out = c;   // returned even on failure so that the caller can read the error text
+  if (rc == KMC_OK && E.set_spill) rc = set_alloc(E);
   if (rc == KMC_OK) rc = engine_reset(E);
   return rc;
 }
@@ -2170,6 +2564,12 @@ void kmcm_destroy(kmcm_ctx* c) {
   if (E.board_host) cudaFreeHost(E.board_host);
   cudaFree(E.ctr);
   cudaFree(E.viol_ring);
+  for (int b = 0; b < 2; ++b) {
+    if (E.set_pinned[b]) cudaFreeHost(E.set_pinned[b]);
+    if (E.set_copied[b]) cudaEventDestroy(E.set_copied[b]);
+    if (E.set_probed[b]) cudaEventDestroy(E.set_probed[b]);
+  }
+  if (E.set_copy_stream) cudaStreamDestroy(E.set_copy_stream);
   for (cudaEvent_t ev : E.event_pool) cudaEventDestroy(ev);
   if (E.ev_begin) cudaEventDestroy(E.ev_begin);
   if (E.ev_end) cudaEventDestroy(E.ev_end);
@@ -2364,8 +2764,9 @@ const char* kmcm_strerror(const kmcm_ctx* c, int code) {
 }
 
 // ---- fingerprint set alone ---------------------------------------------------------------
+// (not with set_spill: the keys in host memory are not consulted, so put() could call a known fingerprint new)
 static int fpset_call(kmcm_ctx* c, const uint64_t* fps, size_t n, uint8_t* out, int insert) {
-  if (!c || (!fps && n) || (!out && n)) return KMC_E_BADARG;
+  if (!c || E.set_spill || (!fps && n) || (!out && n)) return KMC_E_BADARG;
   if (n == 0) return KMC_OK;
   CK(cudaSetDevice(E.device));
   uint64_t* d_fps = nullptr;
@@ -2386,7 +2787,7 @@ int kmcm_fpset_put(kmcm_ctx* c, const uint64_t* fps, size_t n, uint8_t* out_seen
 int kmcm_fpset_contains(kmcm_ctx* c, const uint64_t* fps, size_t n, uint8_t* out) { return fpset_call(c, fps, n, out, 0); }
 int kmcm_fpset_size(const kmcm_ctx* c_, uint64_t* out) {
   kmcm_ctx* c = const_cast<kmcm_ctx*>(c_);
-  if (!c || !out) return KMC_E_BADARG;
+  if (!c || E.set_spill || !out) return KMC_E_BADARG;
   unsigned long long t = 0;
   CK(cudaSetDevice(E.device));
   CK(cudaMemcpy(&t, &E.ctr->store_tail, 8, cudaMemcpyDeviceToHost));
@@ -2395,7 +2796,10 @@ int kmcm_fpset_size(const kmcm_ctx* c_, uint64_t* out) {
 }
 
 // ---- sharded (multi-rank) building blocks -------------------------------------------------
+// None of them runs on a set_spill context: they insert without the filter that keeps the store free of states whose
+// keys are in host memory.
 int kmcm_shard_begin(kmcm_ctx* c) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   int rc = engine_reset(E);
   if (rc) return rc;
@@ -2406,6 +2810,7 @@ int kmcm_shard_begin(kmcm_ctx* c) {
 }
 
 int kmcm_shard_buffers(kmcm_ctx* c, kmc_shard_buffers_t* out) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !out) return KMC_E_BADARG;
   out->cand = E.cand;
   out->region_rows = E.region_rows;
@@ -2417,11 +2822,13 @@ int kmcm_shard_buffers(kmcm_ctx* c, kmc_shard_buffers_t* out) {
 }
 
 int kmcm_shard_seed_init(kmcm_ctx* c) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   return seed_init(E);
 }
 
 int kmcm_shard_expand(kmcm_ctx* c, uint64_t first, uint64_t count) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   if (count > E.chunk_states) {
     E.last_error = "expand chunk larger than chunk_states";
@@ -2432,6 +2839,7 @@ int kmcm_shard_expand(kmcm_ctx* c, uint64_t first, uint64_t count) {
 }
 
 int kmcm_shard_counts(kmcm_ctx* c, uint64_t* host_counts) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !host_counts) return KMC_E_BADARG;
   unsigned long long tmp[MAX_WORLD];
   CK(cudaMemcpyAsync(tmp, E.ctr->cand_count, sizeof(tmp), cudaMemcpyDeviceToHost, E.stream));
@@ -2441,11 +2849,13 @@ int kmcm_shard_counts(kmcm_ctx* c, uint64_t* host_counts) {
 }
 
 int kmcm_shard_reset_cand(kmcm_ctx* c) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   return reset_cand(E);
 }
 
 int kmcm_shard_insert(kmcm_ctx* c, const uint64_t* rows_dev, uint64_t rows, uint64_t* new_tail) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   if (rows) {
     int rc = launch_insert(E, rows_dev, nullptr, rows, rows);
@@ -2462,6 +2872,7 @@ int kmcm_shard_insert(kmcm_ctx* c, const uint64_t* rows_dev, uint64_t rows, uint
 }
 
 int kmcm_shard_level_done(kmcm_ctx* c, uint64_t* level_first, uint64_t* level_count) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   DevCounters h;
   int rc = end_level(E, std::max<uint64_t>(E.level_count * 2, 1024), true, h);
@@ -2473,6 +2884,7 @@ int kmcm_shard_level_done(kmcm_ctx* c, uint64_t* level_first, uint64_t* level_co
 
 // ---- fused exchange over peer memory ---------------------------------------------------------
 int kmcm_shard_ipc_handle(kmcm_ctx* c, void* out64) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !out64 || !E.inbox) return KMC_E_BADARG;
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   cudaIpcMemHandle_t h;
@@ -2483,6 +2895,7 @@ int kmcm_shard_ipc_handle(kmcm_ctx* c, void* out64) {
 }
 
 int kmcm_shard_open_peers(kmcm_ctx* c, const void* handles, uint32_t world) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !handles || world != E.world || !E.inbox) return KMC_E_BADARG;
   CK(cudaSetDevice(E.device));
   for (uint32_t r = 0; r < world; ++r) {
@@ -2503,6 +2916,7 @@ int kmcm_shard_open_peers(kmcm_ctx* c, const void* handles, uint32_t world) {
 // expand a frontier chunk, storing every successor row directly into its owner's inbox, then
 // publish the per-owner row counts into the owners' inbox headers (both on the engine stream)
 int kmcm_shard_expand_p2p(kmcm_ctx* c, uint64_t first, uint64_t count) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   if (count > E.chunk_states) return KMC_E_BADARG;
   int rc = reset_cand(E);
@@ -2520,6 +2934,7 @@ int kmcm_shard_expand_p2p(kmcm_ctx* c, uint64_t first, uint64_t count) {
 
 // seed: the initial states go through the same inbox path (rank 0 contributes them)
 static int seed_p2p(kmcm_ctx* c, bool publish) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   CK(cudaSetDevice(E.device));
   unsigned long long counts[MAX_WORLD] = {0};
@@ -2555,6 +2970,7 @@ int kmcm_shard_seed_p2p(kmcm_ctx* c) { return seed_p2p(c, true); }
 // insert everything the peers stored into the current inbox buffer, then switch buffers.
 // The caller must have put a cross-rank barrier on the stream between expand_p2p and this call.
 int kmcm_shard_insert_p2p(kmcm_ctx* c) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   Params p = E.params();
   {
@@ -2572,6 +2988,7 @@ int kmcm_shard_insert_p2p(kmcm_ctx* c) {
 //   wait until every source is ready for this round; insert from the own inbox; publish done
 // Every rank must call it the same number of times (count = 0 on ranks without work).
 int kmcm_shard_round_p2p(kmcm_ctx* c, uint64_t first, uint64_t count, int seed) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   if (count > E.chunk_states) return KMC_E_BADARG;
   CK(cudaSetDevice(E.device));
@@ -2602,6 +3019,7 @@ int kmcm_shard_round_p2p(kmcm_ctx* c, uint64_t first, uint64_t count, int seed) 
 // for all summaries, copy the board to pinned host memory, ONE stream synchronisation.  board_out receives
 // world x 8 words: {level id, new states, violations, store tail, generated, fail, deadlocks, -} per rank.
 int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !E.peers_open || !board_out) return KMC_E_STATE;
   CK(cudaSetDevice(E.device));
   int rc = launch_invariants(E, E.level_first + E.level_count, std::max<uint64_t>(E.level_count * 2, 1024));
@@ -2649,11 +3067,13 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
 // same-process peers (one context per GPU in one process): direct pointers instead of CUDA IPC handles.
 // inboxes[r] = the value kmcm_shard_inbox_ptr returned for rank r's context.
 int kmcm_shard_inbox_ptr(kmcm_ctx* c, void** out) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !out || !E.inbox_alloc) return KMC_E_BADARG;
   *out = E.inbox_alloc;
   return KMC_OK;
 }
 int kmcm_shard_open_peers_direct(kmcm_ctx* c, void* const* inboxes, const int* devices, uint32_t world) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c || !inboxes || !devices || world != E.world || !E.inbox_alloc) return KMC_E_BADARG;
   CK(cudaSetDevice(E.device));
   for (uint32_t r = 0; r < world; ++r) {
@@ -2673,6 +3093,7 @@ int kmcm_shard_open_peers_direct(kmcm_ctx* c, void* const* inboxes, const int* d
 }
 
 int kmcm_shard_sync(kmcm_ctx* c) {
+  if (c && E.set_spill) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   CK(cudaEventRecord(E.ev_end, E.stream));
   DevCounters h;

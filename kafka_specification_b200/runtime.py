@@ -41,6 +41,8 @@ class Stats(ctypes.Structure):
         ("launches_expand", ctypes.c_uint64), ("launches_insert", ctypes.c_uint64), ("launches_other", ctypes.c_uint64),
         ("wall_ms", ctypes.c_double), ("table_slots", ctypes.c_uint64), ("max_states", ctypes.c_uint64),
         ("complete", ctypes.c_uint64), ("gpu_ms_invariant", ctypes.c_double), ("slot_bytes", ctypes.c_uint64),
+        ("set_flushes", ctypes.c_uint64), ("set_host_keys", ctypes.c_uint64), ("set_filtered", ctypes.c_uint64),
+        ("gpu_ms_set_spill", ctypes.c_double), ("set_link_bytes", ctypes.c_uint64),
     ]
 
     def as_dict(self) -> dict:
@@ -374,7 +376,9 @@ class RunResult:
 
 
 class Checker:
-    """One GPU-resident model checker instance (one ``kmc_ctx``)."""
+    """One GPU-resident model checker instance (one ``kmc_ctx``).  ``options`` are kmc_create's JSON options
+    (include/kspecmc.h), e.g. ``table_log2=27, max_states=N, spill=True, set_spill=True``; ``cont`` stands for
+    ``continue``."""
 
     def __init__(self, model: str, model_lib: str | None = None, model_json: str | None = None, **options):
         self.lib = load_library()

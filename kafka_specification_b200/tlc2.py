@@ -2,7 +2,7 @@
 
     python -m kafka_specification_b200.tlc2 [-config F.cfg] [-workers N|auto] [-deadlock] [-continue]
                                              [-fpbits N] [-maxstates N] [-I dir] [-metadir d] [-checkpoint MIN]
-                                             [-recover DIR] [-spill] [-coverage N] [-tool] SPEC
+                                             [-recover DIR] [-spill] [-setspill] [-coverage N] [-tool] SPEC
 
 ``SPEC`` is a module name or a path to ``SPEC.tla``; modules it EXTENDS / INSTANCEs are resolved
 from the same directory (and ``-I`` directories), like TLC does.  The spec and its ``.cfg`` are
@@ -13,6 +13,8 @@ kmc_create); ``-workers auto`` = one GPU (the GPU grid replaces TLC's worker thr
 messages in TLC's tool-mode markers (``@!@!@STARTMSG code:class @!@!@`` ... ``@!@!@ENDMSG code @!@!@``).
 ``-coverage N`` prints TLC's action-level coverage table ("distinct:generated" per action) once, at the end of the
 run (also after a violation): TLC repeats it every N minutes, but a search here takes seconds.
+``-setspill`` (an extension, like ``-spill``) moves the fingerprint set's keys to host memory whenever its table fills,
+so that a state space larger than the table still finishes (one GPU; see ``set_spill`` in include/kspecmc.h).
 ``-continue`` searches past violations and prints one error block per violated invariant, ordered by (first violating
 level, cfg index), each with the counterexample that ends in the smallest-fingerprint violator of that level; the first
 block is the one a run without ``-continue`` prints.  TLC under ``-continue`` prints a trace for every violating state
@@ -56,6 +58,8 @@ def parse_args(argv):
     ap.add_argument("-recover", help="resume from the checkpoint in this directory")
     ap.add_argument("-spill", action="store_true",
                     help="extension: keep only the live BFS window in HBM and move older levels to host memory")
+    ap.add_argument("-setspill", action="store_true",
+                    help="extension: move the fingerprint set's keys to host memory whenever its HBM table fills")
     ap.add_argument("-tool", action="store_true")
     ap.add_argument("-device", type=int, default=0)
     ap.add_argument("-cleanup", action="store_true")
@@ -218,6 +222,8 @@ def main(argv=None) -> int:
         opts["recover"] = a.recover
     if a.spill:
         opts["spill"] = True
+    if a.setspill:
+        opts["set_spill"] = True
     try:
         ck = Checker(name, **opts)
     except KmcError as e:
