@@ -39,6 +39,17 @@ def bits_for(card: int) -> int:
     return max(0, (card - 1).bit_length())
 
 
+def parse_value(text: str):
+    """A key or enum value as ``fmt`` printed it into a description: quoted text is a string, digits an int, anything
+    else a model value."""
+    if text.startswith('"'):
+        return text[1:-1]
+    try:
+        return int(text)
+    except ValueError:
+        return ModelValue(text)
+
+
 class Atom:
     __slots__ = ("index", "path", "bits", "word", "shift", "card")
 
@@ -57,8 +68,36 @@ class Layout:
         self.atoms: list[Atom] = []
         self.var_types: dict[str, "Ty"] = {}
         self.variables: list[str] = []
+        self.spans: dict[str, tuple[int, int]] = {}      # variable -> the index range [begin, end) of its atoms
         self.words = 0
         self.bits = 0
+
+    def add_variable(self, v: str, ty: "Ty"):
+        """Allocates the atoms of ``v`` after those of the variables added before it."""
+        begin = len(self.atoms)
+        ty.alloc(self, v)
+        self.variables.append(v)
+        self.var_types[v] = ty
+        self.spans[v] = (begin, len(self.atoms))
+
+    @classmethod
+    def from_description(cls, desc: dict) -> "Layout":
+        """The inverse of ``describe()`` (what model.json holds), for decoding: the variables' types are rebuilt, their
+        atoms allocated in variable order and placed at the described word / shift.  A description these types do not
+        allocate atom for atom (a model.json written by another version of the lowering) raises."""
+        lay = cls()
+        for v in desc["variables"]:
+            lay.add_variable(v, ty_from_description(desc["types"][v]))
+        got = [(a.path, a.bits) for a in lay.atoms]
+        want = [(a["path"], a["bits"]) for a in desc["atoms"]]
+        if got != want:
+            i = next((i for i, (g, w) in enumerate(zip(got, want)) if g != w), min(len(got), len(want)))
+            raise LowerError(f"layout description does not match its types: atom {i} is described as "
+                             f"{want[i] if i < len(want) else None}, the types allocate {got[i] if i < len(got) else None}")
+        for a, d in zip(lay.atoms, desc["atoms"]):
+            a.word, a.shift = d["word"], d["shift"]
+        lay.words, lay.bits = desc["words"], desc["bits"]
+        return lay
 
     def new_atom(self, path: str, bits: int, card: int | None = None) -> Atom:
         if bits > 32:
@@ -1215,3 +1254,33 @@ class TSeq(Ty):
                 out[t.atom.index] = "0"
             else:
                 out[t.atom.index] = lw.tmp_int(f"({live.s} ? {code} : 0)")
+
+
+def ty_from_description(d: dict) -> Ty:
+    """The unallocated layout type whose ``describe()`` is ``d``.  Only for decoding: enum gids are list positions."""
+    k = d["t"]
+    if k == "int":
+        return TInt(d["lo"], d["hi"])
+    if k == "bool":
+        return TBool()
+    if k == "enum":
+        vals = [parse_value(x) for x in d["values"]]
+        return TEnum(vals, {x: i for i, x in enumerate(vals)})
+    if k == "rec":
+        return TRec({f: ty_from_description(fd) for f, fd in d["fields"].items()})
+    if k == "fn":           # one type per key: every element allocates its own atoms
+        return TFn([parse_value(x) for x in d["keys"]], [ty_from_description(d["elem"]) for _ in d["keys"]])
+    if k == "prefixfn":
+        return TPrefixFn([parse_value(x) for x in d["keys"]], ty_from_description(d["inner"]), parse_value(d["nil"]),
+                         d["len"])
+    if k == "tuple":
+        return TTuple([ty_from_description(e) for e in d["elems"]])
+    if k == "union":
+        return TUnion([ty_from_description(a) for a in d["alts"]])
+    if k == "set":
+        if d["repr"] == "keyed":
+            return TKeyedSet(ty_from_description(d["elem"]), d["key"])
+        return TSet(ty_from_description(d["elem"]), d.get("cap"), d.get("nonempty", False))
+    if k == "seq":
+        return TSeq(ty_from_description(d["elem"]), d["cap"])
+    raise LowerError(f"layout description has an unknown type {k!r}")

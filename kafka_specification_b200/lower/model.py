@@ -507,7 +507,6 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     ti = TypeInference(lw)
     ti.collect(d.body, dctx, d.module, {})
     lay = L.Layout()
-    lay.variables = list(lw.variables)
     def apply_prefix(ty, arr, length):
         if isinstance(ty, L.TFn):
             for t in ty.elems:
@@ -550,8 +549,7 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
             ty.set_cap(ti.seq_caps[v])
         if v in cfg.prefix:
             apply_prefix(ty, *cfg.prefix[v])
-        lay.var_types[v] = ty
-        ty.alloc(lay, v)
+        lay.add_variable(v, ty)
     lay.finish()
     lw.layout = lay
 

@@ -13,8 +13,8 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from .frontend.cfg import ModelValue
-from .frontend.values import FnVal, fmt
+from .frontend.values import fmt
+from .lower.layout import Layout
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "build")
@@ -144,217 +144,39 @@ def model_paths(name: str) -> tuple[str, str]:
     return os.path.join(d, f"libkmc_{name}.so"), os.path.join(d, "model.json")
 
 
-# ---------------------------------------------------------------------------
-# decoding packed states from model.json (no lowering needed at run time)
-# ---------------------------------------------------------------------------
-def _parse_atom(text: str):
-    if text.startswith('"'):
-        return text[1:-1]
-    try:
-        return int(text)
-    except ValueError:
-        return ModelValue(text)
-
-
-def _bits_for(card: int) -> int:
-    return max(0, (card - 1).bit_length())
-
-
 class StateDecoder:
-    """Rebuilds TLA+ values from packed words using the layout description in model.json."""
+    """Rebuilds TLA+ values from packed words with the lowering's layout types, rebuilt from model.json."""
 
     def __init__(self, meta: dict):
         self.meta = meta
-        self.lay = meta["layout"]
-        self.atoms = self.lay["atoms"]
-        self.variables = self.lay["variables"]
-
-    def _card(self, t) -> int:
-        k = t["t"]
-        if k == "int":
-            return t["hi"] - t["lo"] + 1
-        if k == "bool":
-            return 2
-        if k == "enum":
-            return len(t["values"])
-        if k == "rec":
-            c = 1
-            for f in t["fields"].values():
-                c *= self._card(f)
-            return c
-        if k == "fn":
-            return self._card(t["elem"]) ** len(t["keys"])
-        if k == "tuple":
-            c = 1
-            for e in t["elems"]:
-                c *= self._card(e)
-            return c
-        if k == "union":
-            return sum(self._card(a) for a in t["alts"])
-        if k == "set":
-            return (1 << self._card(t["elem"])) - (1 if t.get("nonempty") else 0)
-        raise ValueError(k)
-
-    def _dec(self, t, code: int):
-        k = t["t"]
-        if k == "int":
-            return code + t["lo"]
-        if k == "bool":
-            return bool(code)
-        if k == "enum":
-            return _parse_atom(t["values"][code])
-        if k == "rec":
-            d = {}
-            for f, ft in t["fields"].items():
-                c = self._card(ft)
-                d[f] = self._dec(ft, code % c)
-                code //= c
-            return FnVal(d)
-        if k == "fn":
-            d = {}
-            c = self._card(t["elem"])
-            for key in t["keys"]:
-                d[_parse_atom(key)] = self._dec(t["elem"], code % c)
-                code //= c
-            return FnVal(d)
-        if k == "tuple":
-            out = []
-            for e in t["elems"]:
-                c = self._card(e)
-                out.append(self._dec(e, code % c))
-                code //= c
-            return tuple(out)
-        if k == "union":
-            off = 0
-            for a in t["alts"]:
-                c = self._card(a)
-                if code < off + c:
-                    return self._dec(a, code - off)
-                off += c
-            raise ValueError("bad union code")
-        if k == "set":
-            c = self._card(t["elem"])
-            if t.get("nonempty"):
-                code += 1
-            return frozenset(self._dec(t["elem"], j) for j in range(c) if (code >> j) & 1)
-        raise ValueError(k)
-
-    def _read(self, t, codes: list[int], pos: list[int]):
-        k = t["t"]
-        if k == "rec":
-            d = {}
-            for f, ft in t["fields"].items():
-                if ft["t"] == "prefixfn":
-                    # entries at index >= the record's length field are the nil value; the others hold the inner code
-                    n, vals = d[ft["len"]], {}
-                    for key in ft["keys"]:
-                        kk = _parse_atom(key)
-                        if _bits_for(self._card(ft["inner"])) == 0:
-                            x = self._dec(ft["inner"], 0)
-                        else:
-                            x = self._dec(ft["inner"], codes[pos[0]])
-                            pos[0] += 1
-                        vals[kk] = x if kk < n else _parse_atom(ft["nil"])
-                    d[f] = FnVal(vals)
-                else:
-                    d[f] = self._read(ft, codes, pos)
-            return FnVal(d)
-        if k == "fn":
-            return FnVal({_parse_atom(key): self._read(t["elem"], codes, pos) for key in t["keys"]})
-        if k == "tuple":
-            return tuple(self._read(e, codes, pos) for e in t["elems"])
-        if k == "seq":
-            n = 0
-            if t["cap"] > 0:
-                n = codes[pos[0]]
-                pos[0] += 1
-            items = []
-            for _ in range(t["cap"]):              # one scalar code per slot (mixed radix for record elements)
-                if _bits_for(self._card(t["elem"])) == 0:
-                    items.append(self._dec(t["elem"], 0))
-                else:
-                    items.append(self._dec(t["elem"], codes[pos[0]]))
-                    pos[0] += 1
-            return tuple(items[:n])
-        if k == "set":
-            if t["repr"] == "keyed":
-                key, fields = t["key"], t["elem"]["fields"]
-                rest = {"t": "rec", "fields": {f: ft for f, ft in fields.items() if f != key}}
-                out = []
-                for j in range(self._card(fields[key])):
-                    c = codes[pos[0]]
-                    pos[0] += 1
-                    if c:
-                        d = dict(self._dec(rest, c - 1).items)
-                        d[key] = self._dec(fields[key], j)
-                        out.append(FnVal({f: d[f] for f in fields}))
-                return frozenset(out)
-            ecard = self._card(t["elem"])
-            if t["repr"] == "bitmap":
-                out, base, n = [], 0, ecard
-                while n > 0:
-                    b = min(32, n)
-                    m = codes[pos[0]]
-                    pos[0] += 1
-                    out += [self._dec(t["elem"], base + j) for j in range(b) if (m >> j) & 1]
-                    base += b
-                    n -= b
-                return frozenset(out)
-            cnt = codes[pos[0]]
-            pos[0] += 1
-            slots = codes[pos[0]: pos[0] + t["cap"]]
-            pos[0] += t["cap"]
-            return frozenset(self._dec(t["elem"], c) for c in slots[:cnt])
-        card = self._card(t)
-        if _bits_for(card) == 0:
-            return self._dec(t, 0)
-        c = codes[pos[0]]
-        pos[0] += 1
-        return self._dec(t, c)
+        self.layout = Layout.from_description(meta["layout"])
+        self.variables = self.layout.variables
 
     def decode(self, words) -> dict:
-        codes = [(int(words[a["word"]]) >> a["shift"]) & ((1 << a["bits"]) - 1) for a in self.atoms]
-        pos = [0]
-        return {v: self._read(self.lay["types"][v], codes, pos) for v in self.variables}
+        return self.layout.py_unpack(words)
 
     def text(self, words) -> str:
         st = self.decode(words)
         return "\n".join(f"/\\ {v} = {fmt(st[v])}" for v in self.variables)
 
-    def _spans(self) -> list[tuple[int, int]]:
-        """Atom index range [begin, end) each variable reads (static: no type consumes a value-dependent number of
-        codes), found by decoding the all-zero code vector once."""
-        if getattr(self, "_span_cache", None) is None:
-            zeros, pos, spans = [0] * len(self.atoms), [0], []
-            for v in self.variables:
-                b = pos[0]
-                self._read(self.lay["types"][v], zeros, pos)
-                spans.append((b, pos[0]))
-            self._span_cache = spans
-        return self._span_cache
-
     def texts(self, rows) -> list[str]:
         """TLC-style text of MANY packed states (rows: [n, W] uint64): the atom codes are extracted with numpy, and
         every variable is decoded once per DISTINCT value it takes in the batch (a few thousand for millions of
         states), so that state-set digests of 10^6..10^7 states take seconds instead of minutes."""
-        rows = np.ascontiguousarray(rows, dtype=np.uint64).reshape(-1, self.lay["words"])
+        lay = self.layout
+        rows = np.ascontiguousarray(rows, dtype=np.uint64).reshape(-1, lay.words)
         n = rows.shape[0]
         if n == 0:
             return []
-        codes = np.empty((n, len(self.atoms)), dtype=np.int64)
-        for i, a in enumerate(self.atoms):
-            codes[:, i] = ((rows[:, a["word"]] >> np.uint64(a["shift"])) & np.uint64((1 << a["bits"]) - 1)).astype(np.int64)
+        codes = np.empty((n, len(lay.atoms)), dtype=np.int64)
+        for a in lay.atoms:
+            codes[:, a.index] = ((rows[:, a.word] >> np.uint64(a.shift)) & np.uint64(a.mask)).astype(np.int64)
         parts = []
-        for v, (b, e) in zip(self.variables, self._spans()):
-            ty = self.lay["types"][v]
-            if e == b:
-                txt = f"/\\ {v} = {fmt(self._read(ty, [], [0]))}"
-                parts.append([txt] * n)
-                continue
+        for v in self.variables:
+            b, e = lay.spans[v]
             uniq, inv = np.unique(codes[:, b:e], axis=0, return_inverse=True)
-            table = [f"/\\ {v} = {fmt(self._read(ty, [int(x) for x in u], [0]))}" for u in uniq]
-            inv = np.asarray(inv).reshape(-1)
-            parts.append([table[j] for j in inv])
+            table = [f"/\\ {v} = {fmt(lay.var_types[v].py_read(dict(zip(range(b, e), map(int, u)))))}" for u in uniq]
+            parts.append([table[j] for j in np.asarray(inv).reshape(-1)])
         return ["\n".join(p) for p in zip(*parts)]
 
 

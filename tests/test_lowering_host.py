@@ -4,6 +4,7 @@ This exercises exactly the header the CUDA engine includes (same expand / invari
 code, same packed layout) on a machine without a GPU.  The harness (tests/support/host_model.cpp)
 is test infrastructure: no product path runs on the CPU.
 """
+import json
 import os
 
 import numpy as np
@@ -12,6 +13,8 @@ import pytest
 from conftest import REFERENCE, ROOT, needs_reference
 from golden.make_golden import state_digest
 from hostmodel import lower_model, run_host
+from kafka_specification_b200.build import registry as build_registry, tla_search_dirs
+from kafka_specification_b200.lower.layout import Layout
 
 DIRS = [REFERENCE, os.path.join(ROOT, "models")]
 
@@ -77,13 +80,46 @@ def test_layout_roundtrip_and_init(registry):
     assert m.words == lay.words and len(m.init_states) == 1
     st = m.decode_state(m.init_states[0])
     assert lay.py_pack(st) == m.init_states[0]
-    # the runtime decoder (model.json only) agrees with the lowering's own decoder
+    # the runtime decoder (the layout rebuilt from model.json alone) agrees with the lowering's own layout
     from kafka_specification_b200.runtime import StateDecoder
     dec = StateDecoder(m.meta())
     r = run_host(m, dump=True, max_states=5000)
     for row in r["states"][:500]:
         assert dec.decode(row) == m.decode_state(row)
         assert lay.py_pack(m.decode_state(row)) == [int(x) for x in row]
+
+
+@needs_reference
+@pytest.mark.parametrize("name", sorted(build_registry()))
+def test_layout_rebuilt_from_its_description(name):
+    """Layout.from_description (what decodes model.json at run time) gives back the lowering's layout: the same
+    description, the same atoms and the same decoded initial states."""
+    spec = build_registry()[name]
+    with open(os.path.join(ROOT, spec["cfg"])) as f:
+        m = lower_model(spec["module"], tla_search_dirs(), f.read(), name=name)
+    lay = m.lowerer.layout
+    back = Layout.from_description(json.loads(json.dumps(lay.describe())))
+    assert back.describe() == lay.describe()
+    assert [(a.path, a.bits, a.word, a.shift) for a in back.atoms] == [(a.path, a.bits, a.word, a.shift) for a in lay.atoms]
+    for words in m.init_states:
+        assert back.py_unpack(words) == lay.py_unpack(words)
+
+
+def test_layout_description_of_other_atoms_is_rejected():
+    """A model.json whose atoms the layout types do not allocate (one written by another version of the lowering)
+    raises instead of decoding wrongly."""
+    from kafka_specification_b200.lower.svals import LowerError
+    specs = os.path.join(ROOT, "tests", "specs")
+    desc = lower_model("MiniQueue", [specs], open(os.path.join(specs, "MiniQueue.cfg")).read()).layout
+    Layout.from_description(desc)
+    wider = json.loads(json.dumps(desc))
+    wider["atoms"][0]["bits"] += 1
+    with pytest.raises(LowerError, match="atom 0"):
+        Layout.from_description(wider)
+    shorter = json.loads(json.dumps(desc))
+    shorter["atoms"].pop()
+    with pytest.raises(LowerError, match=f"atom {len(shorter['atoms'])}"):
+        Layout.from_description(shorter)
 
 
 @needs_reference
