@@ -18,6 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
+from kafka_specification_b200.build import registry, tla_search_dirs  # noqa: E402
 from kafka_specification_b200.lower.model import LoweredModel, lower_model  # noqa: E402,F401
 
 BUILD = os.path.join(ROOT, "build", "hosttest")
@@ -81,6 +82,15 @@ def _library_path(header_text: str, invariants_text: str) -> str:
 
 
 @functools.lru_cache(maxsize=None)
+def lower_registered(name: str) -> LoweredModel:
+    """The registered model `name` (build.registry()) lowered from its module and cfg as build() lowers it, once per
+    process; `lower_registered.__wrapped__(name)` lowers it afresh."""
+    spec = registry()[name]
+    with open(os.path.join(ROOT, spec["cfg"])) as f:
+        return lower_model(spec["module"], tla_search_dirs(), f.read(), name=name)
+
+
+@functools.lru_cache(maxsize=None)
 def _load(so: str) -> ctypes.CDLL:
     lib = ctypes.CDLL(so)
     for fn, (res, args) in SIGNATURES.items():
@@ -110,6 +120,11 @@ class HostModel:
     @classmethod
     def from_lowered(cls, model: LoweredModel):
         return cls(model.name, model.header, model.invariants_header)
+
+    @classmethod
+    def for_registered(cls, name: str):
+        """The headers lower_registered(name) lowers, without build/."""
+        return cls.from_lowered(lower_registered(name))
 
     @classmethod
     def for_built_model(cls, name: str):

@@ -4,7 +4,8 @@ TLC's rule for the action of a successor (the one its -coverage report and its e
 user-defined operator applied below ``Next``.  ``run_bfs_by_action`` runs Oracle A's own BFS unchanged and counts,
 per action, the successors generated -- duplicates and successors a CONSTRAINT discards included, exactly as
 "generated" counts them.  The lowering labels its emit sites by the same rule in its own code path, so the two
-agreeing checks the lowering's labels against an independent interpreter.
+agreeing checks the lowering's labels against an independent interpreter.  ``OracleA`` holds the labelled interpreter
+of one registered model and replays the error traces of GPU runs through it.
 """
 from __future__ import annotations
 
@@ -108,6 +109,49 @@ class LabelledInterp(tla_interp.Interp):
             return
         if self.ev_bool(e, ctx, fm, env, st, st1):
             self._next_l(rest, st, st1, out, label)
+
+
+class OracleA:
+    """Oracle A's interpreter for one registered model: initial states, labelled successors, predicates."""
+
+    def __init__(self, name: str):
+        from kafka_specification_b200.build import registry, tla_search_dirs
+        from kafka_specification_b200.frontend.cfg import parse_cfg
+        from kafka_specification_b200.frontend.modules import load_root
+        spec = registry()[name]
+        with open(os.path.join(ROOT, spec["cfg"])) as f:
+            self.cfg = parse_cfg(f.read())
+        root = load_root(spec["module"], tla_search_dirs())
+        self.it = LabelledInterp(root, self.cfg)
+        init_e, self.next_e = tla_interp.resolve_init_next(root, self.cfg)
+        self.inits = self.it.init_states(init_e)
+
+    def text(self, st: dict) -> str:
+        from kafka_specification_b200.frontend.values import fmt
+        return "\n".join(f"/\\ {v} = {fmt(st[v])}" for v in self.it.variables)
+
+    def holds(self, name: str, st: dict) -> bool:
+        return self.it.eval_named_predicate(name, st)
+
+    def violated(self, st: dict) -> list[str]:
+        return [inv for inv in self.cfg.invariants if not self.holds(inv, st)]
+
+    def in_model(self, st: dict) -> bool:
+        return all(self.holds(c, st) for c in self.cfg.constraints)
+
+    def replay(self, trace: list[dict]) -> list[dict]:
+        """The Oracle A states of an error trace (entries with "text" and "action"): the first one an initial state of
+        that text, each next one a successor of its predecessor under the action the trace names, of that text."""
+        assert trace[0]["action"] is None
+        by_text = {self.text(s): s for s in self.inits}
+        assert trace[0]["text"] in by_text, "the first state is not an initial state"
+        states = [by_text[trace[0]["text"]]]
+        for i, t in enumerate(trace[1:], start=1):
+            nxt = [s1 for s1, label in self.it.labelled_successors(self.next_e, states[-1])
+                   if label == t["action"]["name"] and self.text(s1) == t["text"]]
+            assert nxt, f"trace state {i + 1} is not a {t['action']['name']} successor of state {i}:\n{t['text']}"
+            states.append(nxt[0])
+        return states
 
 
 def run_bfs_by_action(module: str, search_dirs: list[str], cfg_text: str) -> dict:

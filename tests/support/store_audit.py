@@ -275,7 +275,8 @@ def copy_parents(ck, first: int, count: int) -> np.ndarray:
 
 def audit_checker(ck, levels: list[int], distinct: int, *, check_deadlock: bool | None = None, audit: AuditLib | None = None) -> dict:
     """Audit the store of a Checker after a run: `levels` are the widths of the levels the run expanded (RunResult /
-    ShardedResult .levels), `distinct` the stored states; the states past the expanded levels are the queue."""
+    ShardedResult .levels), `distinct` the stored states; the states past the expanded levels are the queue.  The
+    report holds the audit's totals and pick, the store and the run's kmc_violation_record (None without a violation)."""
     a = audit or AuditLib.for_built_model(ck.meta["name"])
     if a.digest != ck.meta["digest"]:
         raise AuditError(f"digest: the audit's model.h ({a.digest}) is not the loaded library's ({ck.meta['digest']})")
@@ -286,6 +287,29 @@ def audit_checker(ck, levels: list[int], distinct: int, *, check_deadlock: bool 
         widths.append(distinct - sum(widths))
     cd = a.check_deadlock if check_deadlock is None else check_deadlock
     found = a.check_store(states, parents, widths, len(levels), check_deadlock=cd)
+    record = ck.violation_record() if ck.violation() else None
     want = compare(a, found, stats=ck.stats(), coverage=ck.coverage(), parents=parents, violation=ck.violation(),
-                   record=ck.violation_record() if ck.violation() else None, invariants=ck.meta["invariants"])
-    return {"found": found, "violation": want, "states": states, "parents": parents, "widths": widths}
+                   record=record, invariants=ck.meta["invariants"])
+    return {"found": found, "violation": want, "states": states, "parents": parents, "widths": widths, "record": record}
+
+
+def host_audit(name: str, sites: bool = True) -> tuple[AuditLib, dict, dict]:
+    """The audit of the store that a host BFS of the registered model `name` writes: (AuditLib, the store, the audit's
+    findings)."""
+    a = AuditLib.for_registered(name)
+    st = a.host_bfs(sites=sites)
+    found = a.check_store(st["states"], st["parents"], st["widths"], st["n_expanded"], check_deadlock=a.check_deadlock)
+    return a, st, found
+
+
+def expected_orbit(a: AuditLib, found: dict) -> tuple[list[int], int]:
+    """The counterexample the documented rule picks, as an orbit: (canonical words, fingerprint of the canonical form),
+    computed from the violators alone -- whichever member of each orbit a store happens to hold."""
+    w = a.words
+    rows = found["violators"]
+    dead = rows[:, w + 1] == np.uint64(M64)
+    canon = a.canonicalize(rows[:, :w])
+    fps = fingerprint(canon, a.state_bits)
+    keys = [(0 if d else 1, int(f)) for d, f in zip(dead, fps)]
+    best = min(range(len(rows)), key=lambda i: keys[i])
+    return [int(x) for x in canon[best]], int(fps[best])

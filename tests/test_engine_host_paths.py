@@ -3,23 +3,23 @@ that cross the host spill and the ring wrap, and recovery of a committed checkpo
 
 tests/golden/checkpoint_kip320_n2/ is a bounded checkpoint of kip320_n2 (stop_after_states=2000: written at the end of
 level 9, 2,033 states), kept to show that recover still reads the checkpoint format byte for byte."""
+import functools
 import json
 import os
 
 import numpy as np
 import pytest
 
+import gpu_runs
 from conftest import ROOT
+from gpu_runs import sorted_rows
+from store_audit import copy_parents
 
 pytestmark = pytest.mark.gpu
 
 CHECKPOINT = os.path.join(ROOT, "tests", "golden", "checkpoint_kip320_n2")
 
-
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 22)
-    return Checker(name, **kw)
+checker = functools.partial(gpu_runs.checker, table_log2=22)
 
 
 def sharded(name, cont=False):
@@ -64,17 +64,6 @@ def test_shard_building_blocks_stop_at_the_violation_kmc_run_finds():
     assert s.violation["trace_len"] == len(s.trace) == a.violation["trace_len"] == len(a.trace)
 
 
-def _copy_parents(ck, first, count):
-    buf = np.empty(count, dtype=np.uint64)
-    if count:
-        ck._check(ck.lib.kmc_copy_parents(ck.ctx, first, count, buf.ctypes.data))
-    return buf
-
-
-def _sorted_rows(rows):
-    return rows[np.lexsort(rows.T[::-1])] if len(rows) else rows
-
-
 def test_spill_range_reads_across_the_host_spill_and_the_ring_wrap():
     """262,144 ring slots; the run stops after level 17, whose expansion spilled [0, 390,625) to the host and left the
     device window [390,625, 554,938), which wraps at 524,288.  One read of everything equals reads split across both
@@ -86,10 +75,10 @@ def test_spill_range_reads_across_the_host_spill_and_the_ring_wrap():
         base = sum(r.levels[:-1])              # the last expanded level starts the device window
         assert not r.complete and base < ring * 2 < n and n - base <= ring
         cuts = [0, base - 1000, base + 1000, 2 * ring - 1000, 2 * ring + 1000, n]
-        states, parents = ck.copy_states(0, n), _copy_parents(ck, 0, n)
+        states, parents = ck.copy_states(0, n), copy_parents(ck, 0, n)
         pieces = list(zip(cuts, cuts[1:]))
         assert np.array_equal(states, np.concatenate([ck.copy_states(a, b - a) for a, b in pieces]))
-        assert np.array_equal(parents, np.concatenate([_copy_parents(ck, a, b - a) for a, b in pieces]))
+        assert np.array_equal(parents, np.concatenate([copy_parents(ck, a, b - a) for a, b in pieces]))
     with checker("kip320_small", stop_after_states=500_000) as ck:
         q = ck.run()
         plain = ck.copy_states(0, q.distinct)
@@ -97,7 +86,7 @@ def test_spill_range_reads_across_the_host_spill_and_the_ring_wrap():
     bounds = np.concatenate([[0], np.cumsum(r.levels + [r.queue])])
     assert bounds[-1] == n
     for a, b in zip(bounds, bounds[1:]):
-        assert np.array_equal(_sorted_rows(states[a:b]), _sorted_rows(plain[a:b]))
+        assert np.array_equal(sorted_rows(states[a:b]), sorted_rows(plain[a:b]))
 
 
 @pytest.mark.parametrize("spill", [False, True])

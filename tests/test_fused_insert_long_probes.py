@@ -3,7 +3,7 @@ many rows walk several buckets before their CAS while the expansion goes on.  Th
 the two-kernel pipeline: counts, level widths, successors per emit site and each level's set of states."""
 import pytest
 
-from test_fused_expand_insert import _compare, fused_run, two_kernel_run
+from gpu_runs import compare_runs, fused_run, two_kernel_run
 
 pytestmark = pytest.mark.gpu
 
@@ -12,5 +12,5 @@ def test_fused_run_on_a_loaded_set_matches_two_kernel_pipeline():
     # the store gets its own size: by default it holds half as many states as the set has slots, fewer than 737,794
     kw = {"table_log2": 20, "max_states": 1 << 20}
     fused = fused_run("kip320_small", cont=True, **kw)
-    assert fused[0]["distinct"] == 737_794
-    _compare("kip320_small", fused, two_kernel_run("kip320_small", cont=True, **kw))
+    assert fused[0]["distinct"] == 737_794 and fused[0]["levels"]
+    compare_runs(fused, two_kernel_run("kip320_small", cont=True, **kw))

@@ -4,29 +4,19 @@ Run on an H100:  python -m pytest tests -m gpu -x -q
 Nothing here reads the .tla sources: models are prebuilt (build/models/*), goldens are committed
 (tests/golden/goldens.json), Oracle B compiles from oracle/ with gcc.
 """
-import ctypes
+import functools
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import gpu_runs
 from conftest import ROOT
+from gpu_runs import ALL_MODELS, DIGEST_MODELS, VIOLATING_MODELS, assert_oracle_b_trace
 
 pytestmark = pytest.mark.gpu
 
-ALL_MODELS = ["idsequence", "frl_tiny", "frl_3x4x2", "frl_3x4x3", "kip320_n2", "trunchw_n2", "kip101_n2", "kip279_n2",
-              "firsttry_n2", "kip320_small", "trunchw_small", "kip101_small", "kip279_small", "firsttry_small",
-              "asyncisr_v2", "asyncisr_small", "kip320sym_n2", "kip320sym_small", "minilock", "kip320_with279_small",
-              "asyncisr_w3"]
-DIGEST_MODELS = ["minilock", "idsequence", "frl_tiny", "kip320_n2", "trunchw_n2", "kip101_n2", "kip279_n2", "firsttry_n2",
-                 "asyncisr_v2", "asyncisr_small", "kip320_small", "frl_3x4x2", "frl_3x4x3"]
-
-
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 24)
-    return Checker(name, **kw)
+checker = functools.partial(gpu_runs.checker, table_log2=24)
 
 
 @pytest.mark.parametrize("name", ALL_MODELS)
@@ -83,7 +73,7 @@ def test_stop_at_first_violation_and_trace():
         assert not r.complete and r.violation["kind"] == "invariant"
         assert r.violation["invariant"] in ("WeakIsr", "StrongIsr") and r.violation["level"] == 9
         assert len(r.trace) == 9 and r.trace[0]["action"] is None
-        _assert_trace_is_behaviour("trunchw_small", r.trace, ck)
+        assert_oracle_b_trace("trunchw_small", r.trace, ck.decoder, ck.meta["invariants"])
         assert r.queue > 0
 
 
@@ -162,27 +152,7 @@ def test_probe_count_matches_generated(goldens):
     assert r.generated <= r.stats["probes"] <= 1.05 * r.generated
 
 
-def _assert_trace_is_behaviour(name, trace, ck):
-    """Every step of the error trace is re-checked against ORACLE B (the hand-written C restatement of the spec,
-    independent of the front end and of the lowering): the first state is its Init, each state is among the
-    successors its Next enumerates for the previous one, and the last state violates the reported invariant
-    there too.  (Round 1 validated the steps with the lowered header itself, which a lowering bug would pass.)"""
-    import json
-    import kso
-    reg = json.load(open(os.path.join(ROOT, "models", "MODELS.json")))[name]
-    model, params = reg["kso"]
-    states = [ck.decoder.decode(t["words"]) for t in trace]
-    replicas = sorted(states[0]["replicaLog"].domain(), key=str)
-    recs = [kso.kstate_from_tla(st, replicas) for st in states]
-    assert recs[0] == kso.init_state(model, params), "trace does not start in the oracle's initial state"
-    for i, (a, b) in enumerate(zip(recs, recs[1:])):
-        assert b in kso.successors(model, params, a), f"trace step {i + 1} -> {i + 2} is not a successor under Oracle B"
-    assert kso.violated(model, params, recs[-1], ck.meta["invariants"]), "last trace state violates nothing under Oracle B"
-    for a in recs[:-1]:
-        assert not kso.violated(model, params, a, ck.meta["invariants"]), "an earlier trace state already violates"
-
-
-@pytest.mark.parametrize("name", ["trunchw_small", "kip101_small", "kip279_small", "firsttry_small", "kip320_with279_small"])
+@pytest.mark.parametrize("name", VIOLATING_MODELS)
 def test_error_traces_are_behaviours_under_oracle_b(name, goldens):
     """Default run (stop at the first violation) of every protocol variant the reference says is broken:
     shortest counterexample, each step validated by Oracle B."""
@@ -193,7 +163,7 @@ def test_error_traces_are_behaviours_under_oracle_b(name, goldens):
         assert not r.complete and r.violation["kind"] == "invariant" and r.violation["level"] == first
         assert len(r.trace) == first and r.trace[0]["action"] is None
         assert all(t["action"] is not None for t in r.trace[1:])
-        _assert_trace_is_behaviour(name, r.trace, ck)
+        assert_oracle_b_trace(name, r.trace, ck.decoder, ck.meta["invariants"])
 
 
 def test_kip320_needs_its_epoch_check_as_the_reference_says(goldens):
@@ -283,7 +253,7 @@ def test_error_trace_through_spilled_levels(goldens):
     with checker("trunchw_small", spill=True, max_states=1 << 15) as ck:
         r = ck.run()
         assert not r.complete and r.violation["level"] == first and len(r.trace) == first
-        _assert_trace_is_behaviour("trunchw_small", r.trace, ck)
+        assert_oracle_b_trace("trunchw_small", r.trace, ck.decoder, ck.meta["invariants"])
 
 
 def test_checkpoint_and_recover(tmp_path, goldens):
@@ -386,7 +356,7 @@ def test_two_gpu_violation_and_cross_rank_trace(mode, goldens):
     assert len({t["rank"] for t in r["trace"]}) == 2
     with checker("trunchw_small") as ck:
         trace = [{"words": t["words"]} for t in r["trace"]]
-        _assert_trace_is_behaviour("trunchw_small", trace, ck)
+        assert_oracle_b_trace("trunchw_small", trace, ck.decoder, ck.meta["invariants"])
     # and the full search past the violation still matches the golden
     r = _torchrun([os.path.join(ROOT, "tools", "sharded_check.py"), "trunchw_small", mode, "cont"], 29543 if mode == "p2p" else 29544)
     assert (r["distinct"], r["generated"], r["depth"], r["levels"]) == (g["distinct"], g["generated"], g["depth"], g["levels"])

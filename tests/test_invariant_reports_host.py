@@ -5,24 +5,11 @@ import random
 
 import pytest
 
-from conftest import REFERENCE, ROOT, needs_reference
-from hostmodel import HostModel, lower_model
+from conftest import ROOT, needs_reference
+from hostmodel import HostModel, lower_model, lower_registered
+from kafka_specification_b200.build import registry, tla_search_dirs
 
-DIRS = [REFERENCE, os.path.join(ROOT, "models"), os.path.join(ROOT, "tests", "specs")]
-
-
-def _registry():
-    from kafka_specification_b200.build import registry
-    return registry()
-
-
-def _lower(name):
-    spec = _registry()[name]
-    with open(os.path.join(ROOT, spec["cfg"])) as f:
-        return lower_model(spec["module"], DIRS, f.read(), name=name)
-
-
-ORACLE_A_MODELS = sorted(n for n, s in _registry().items() if s.get("oracle_a"))
+ORACLE_A_MODELS = sorted(n for n, s in registry().items() if s.get("oracle_a"))
 
 
 @needs_reference
@@ -31,7 +18,7 @@ def test_host_bfs_by_mask_gives_every_first_violation_level(name, goldens):
     """A host BFS of the lowered model that checks states through violated_invariants() finds each invariant's first
     violating level as the goldens record it (Oracle A's, and Oracle B's where it ran), constraint-discarded violators
     included; and on every checked state the mask agrees with first_violated_invariant."""
-    m = _lower(name)
+    m = lower_registered(name)
     rep = HostModel.from_lowered(m).invariant_report(m.invariants)
     assert rep.pop(None) == 0, "violated_invariants and first_violated_invariant disagree on a checked state"
     want = {i: l for i, l in goldens[name]["first_violation_level"].items() if l is not None}
@@ -44,10 +31,10 @@ def test_host_bfs_by_mask_gives_every_first_violation_level(name, goldens):
 def test_two_invariants_at_one_level_and_a_discarded_only_violation(goldens):
     """minibound_mixed breaks NotOver and OneFull at level 3; asyncisr_bounded breaks VersionInBound only through
     successors its CONSTRAINT discards (the stored states never violate it)."""
-    mixed = _lower("minibound_mixed")
+    mixed = lower_registered("minibound_mixed")
     rep = HostModel.from_lowered(mixed).invariant_report(mixed.invariants)
     assert rep["NotOver"]["level"] == rep["OneFull"]["level"] == 3
-    m = _lower("asyncisr_bounded")
+    m = lower_registered("asyncisr_bounded")
     hm = HostModel.from_lowered(m)
     rep = hm.invariant_report(m.invariants)
     assert rep["VersionInBound"]["level"] == goldens["asyncisr_bounded"]["first_violation_level"]["VersionInBound"]
@@ -67,12 +54,11 @@ def test_mask_on_random_walks_matches_oracle_a_and_first_violated(name, walks, s
     import tla_interp
     from kafka_specification_b200.frontend.cfg import parse_cfg
     from kafka_specification_b200.frontend.modules import load_root
-    spec = _registry()[name]
-    cfg_text = open(os.path.join(ROOT, spec["cfg"])).read()
-    m = lower_model(spec["module"], DIRS, cfg_text, name=name)
+    spec = registry()[name]
+    m = lower_registered(name)
     hm = HostModel.from_lowered(m)
-    cfg = parse_cfg(cfg_text)
-    it = tla_interp.Interp(load_root(spec["module"], DIRS), cfg)
+    cfg = parse_cfg(open(os.path.join(ROOT, spec["cfg"])).read())
+    it = tla_interp.Interp(load_root(spec["module"], tla_search_dirs()), cfg)
     rng = random.Random(20260923 + len(name))
     inits = list(hm.init_states())
     for _ in range(walks):
@@ -95,15 +81,16 @@ def test_mask_on_random_walks_matches_oracle_a_and_first_violated(name, walks, s
 def test_more_than_64_invariants_lower_without_a_mask():
     """A cfg with 65 INVARIANT entries lowers and runs as before (model.h does not depend on invariants.h); its
     invariants.h says there is no mask, and the engine then reports no per-invariant results (KMC_E_BADARG)."""
-    spec = _registry()["minibound_mixed"]
+    spec = registry()["minibound_mixed"]
     cfg_text = open(os.path.join(ROOT, spec["cfg"])).read() + "\nINVARIANT\n" + "\n".join(["TypeOk"] * 65) + "\n"
-    m = lower_model(spec["module"], DIRS, cfg_text, name="minibound_65")
+    m = lower_model(spec["module"], tla_search_dirs(), cfg_text, name="minibound_65")
     assert len(m.invariants) > 64
     assert "HAS_INVARIANT_MASK = false" in m.invariants_header
     assert "violated_invariants" not in m.header and "first_violated_invariant" in m.header
-    small = _lower("minibound_mixed")
+    lower_afresh = lower_registered.__wrapped__           # two lowerings, not the cached one twice
+    small = lower_afresh("minibound_mixed")
     assert "HAS_INVARIANT_MASK = true" in small.invariants_header
-    assert small.meta() == _lower("minibound_mixed").meta() and "invariants_header" not in small.meta()
+    assert small.meta() == lower_afresh("minibound_mixed").meta() and "invariants_header" not in small.meta()
 
 
 def _trace(n):

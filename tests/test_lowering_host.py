@@ -10,13 +10,11 @@ import os
 import numpy as np
 import pytest
 
-from conftest import REFERENCE, ROOT, needs_reference
+from conftest import ROOT, needs_reference
 from golden.make_golden import state_digest
-from hostmodel import lower_model, run_host
-from kafka_specification_b200.build import registry as build_registry, tla_search_dirs
+from hostmodel import lower_model, lower_registered, run_host
+from kafka_specification_b200.build import registry, tla_search_dirs
 from kafka_specification_b200.lower.layout import Layout
-
-DIRS = [REFERENCE, os.path.join(ROOT, "models")]
 
 SMALL = ["idsequence", "frl_tiny", "frl_3x4x2", "kip320_n2", "trunchw_n2", "kip101_n2", "kip279_n2", "firsttry_n2",
          "asyncisr_v2", "asyncisr_small", "kip320sym_n2"]
@@ -26,16 +24,11 @@ if os.environ.get("KSPEC_SLOW_TESTS") == "1":
     MEDIUM.append("frl_3x4x3")       # 28 M successors on the sequential host harness: 2 more minutes (digest verified once, round 2)
 
 
-def _lower(registry, name):
-    spec = registry[name]
-    return lower_model(spec["module"], DIRS, open(os.path.join(ROOT, spec["cfg"])).read(), name=name)
-
-
 @needs_reference
 @pytest.mark.parametrize("name", SMALL)
-def test_lowered_model_matches_golden_state_for_state(name, goldens, registry):
+def test_lowered_model_matches_golden_state_for_state(name, goldens):
     g = goldens[name]
-    m = _lower(registry, name)
+    m = lower_registered(name)
     assert not m.warnings
     r = run_host(m, dump=True, max_states=200000)
     assert r["fail"] == 0 and r["complete"]
@@ -56,13 +49,13 @@ def test_lowered_model_matches_golden_state_for_state(name, goldens, registry):
 
 @needs_reference
 @pytest.mark.parametrize("name", MEDIUM)
-def test_lowered_model_matches_golden_counts(name, goldens, registry):
+def test_lowered_model_matches_golden_counts(name, goldens):
     """The 3-replica models (10^5..10^6 states): counts against the golden and -- where Oracle A, the interpreter of the
     unchanged .tla text, has been run over the model (hours of Python, tests/golden/run_oracle_a.py) -- the reachable
     state SET, decoded to TLC text, against its order-independent digest."""
     from kafka_specification_b200.runtime import StateDecoder
     g = goldens[name]
-    m = _lower(registry, name)
+    m = lower_registered(name)
     want_digest = "state_digest" in g
     r = run_host(m, max_states=3_000_000, dump=want_digest)
     for k in ("distinct", "generated", "depth", "levels", "deadlocks"):
@@ -74,8 +67,8 @@ def test_lowered_model_matches_golden_counts(name, goldens, registry):
 
 
 @needs_reference
-def test_layout_roundtrip_and_init(registry):
-    m = _lower(registry, "kip320_small")
+def test_layout_roundtrip_and_init():
+    m = lower_registered("kip320_small")
     lay = m.lowerer.layout
     assert m.words == lay.words and len(m.init_states) == 1
     st = m.decode_state(m.init_states[0])
@@ -90,13 +83,11 @@ def test_layout_roundtrip_and_init(registry):
 
 
 @needs_reference
-@pytest.mark.parametrize("name", sorted(build_registry()))
+@pytest.mark.parametrize("name", sorted(registry()))
 def test_layout_rebuilt_from_its_description(name):
     """Layout.from_description (what decodes model.json at run time) gives back the lowering's layout: the same
     description, the same atoms and the same decoded initial states."""
-    spec = build_registry()[name]
-    with open(os.path.join(ROOT, spec["cfg"])) as f:
-        m = lower_model(spec["module"], tla_search_dirs(), f.read(), name=name)
+    m = lower_registered(name)
     lay = m.lowerer.layout
     back = Layout.from_description(json.loads(json.dumps(lay.describe())))
     assert back.describe() == lay.describe()
@@ -123,11 +114,11 @@ def test_layout_description_of_other_atoms_is_rejected():
 
 
 @needs_reference
-def test_pinning_preserves_tlc_multiplicity(registry):
+def test_pinning_preserves_tlc_multiplicity():
     """Kip279.tla:47-51 and Kip320.tla:82-83 generate the same successor twice; 'generated' counts both."""
     import kso
     for name, model in (("kip279_n2", "kip279"), ("kip320_n2", "kip320")):
-        m = _lower(registry, name)
+        m = lower_registered(name)
         assert run_host(m)["generated"] == kso.run(model, [2, 2, 2, 2], max_states=100000)["generated"]
 
 
@@ -138,7 +129,7 @@ def test_layout_overflow_is_trapped():
 INIT Init NEXT Next INVARIANT TypeOk CHECK_DEADLOCK FALSE
 \\* kspec: CAPACITY leaderAndIsrRequests = 1
 """
-    m = lower_model("Kip320", DIRS, cfg, name="kip320_narrow")
+    m = lower_model("Kip320", tla_search_dirs(), cfg, name="kip320_narrow")
     r = run_host(m)
     assert r["fail"] == 1 and not r["complete"]
 
@@ -149,35 +140,36 @@ def test_unbounded_layout_is_rejected():
     cfg = """CONSTANTS Replicas = {r1, r2} Leader = r1 MaxOffset = 1
 INIT Init NEXT Next INVARIANT ValidHighWatermark CHECK_DEADLOCK FALSE"""
     with pytest.raises(LowerError):
-        lower_model("AsyncIsr", DIRS, cfg)       # TypeOk uses Nat (AsyncIsr.tla:42-55): needs a LAYOUT operator
+        # TypeOk uses Nat (AsyncIsr.tla:42-55): needs a LAYOUT operator
+        lower_model("AsyncIsr", tla_search_dirs(), cfg)
 
 
 @needs_reference
 def test_false_assume_is_rejected():
     from kafka_specification_b200.lower.svals import LowerError
     with pytest.raises(LowerError):              # AsyncIsr.tla:27-29: MaxOffset > 0
-        lower_model("MCAsyncIsr", DIRS, open(os.path.join(ROOT, "models", "MCAsyncIsr.cfg")).read().replace(
+        lower_model("MCAsyncIsr", tla_search_dirs(), open(os.path.join(ROOT, "models", "MCAsyncIsr.cfg")).read().replace(
             "MaxOffset = 2", "MaxOffset = 0"))
 
 
 @needs_reference
 @pytest.mark.parametrize("name", ["frl_tiny", "kip320_n2", "kip279_n2", "firsttry_n2", "asyncisr_v2", "kip320_small"])
-def test_two_phase_item_form_equals_expand(name, goldens, registry):
+def test_two_phase_item_form_equals_expand(name, goldens):
     """item_guard/item_body (what the CUDA expand kernel runs) enumerate exactly expand()'s successors."""
     g = goldens[name]
-    m = _lower(registry, name)
+    m = lower_registered(name)
     r = run_host(m, max_states=3_000_000, items=True)
     for k in ("distinct", "generated", "depth", "levels", "deadlocks"):
         assert r[k] == g[k], k
 
 
 @needs_reference
-def test_symmetry_reduction_counts_orbits(goldens, registry):
+def test_symmetry_reduction_counts_orbits(goldens):
     """SYMMETRY Permutations(Replicas): the set holds one representative per orbit; the orbit count
     lies between |states| / n! and |states|, and every count equals both oracles'."""
     full, sym = goldens["kip320_small"], goldens["kip320sym_small"]
     assert full["distinct"] / 6 <= sym["distinct"] < full["distinct"]
     assert sym["depth"] == full["depth"]
-    m = _lower(registry, "kip320sym_small")
+    m = lower_registered("kip320sym_small")
     r = run_host(m, max_states=1_000_000)
     assert (r["distinct"], r["generated"], r["levels"]) == (sym["distinct"], sym["generated"], sym["levels"])

@@ -1,44 +1,15 @@
 """N > 1 path on CPU: the fingerprint-sharded driver (kafka_specification_b200/sharded.py) with
 torch.distributed/gloo, world_size 2 and 3, over a host stand-in for the per-rank engine."""
-import json
-import os
-import socket
-import subprocess
-import sys
-
 import pytest
 
-from conftest import ROOT
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _run(name, world, chunk, tmp_path, extra=()):
-    if not os.path.exists(os.path.join(ROOT, "build", "models", name, "model.h")):
-        pytest.skip(f"lowered model {name} not built")
-    out = str(tmp_path / f"{name}_{world}.json")
-    port = _free_port()
-    procs = []
-    for rank in range(world):
-        env = dict(os.environ, RANK=str(rank), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "support", "gloo_worker.py"),
-                                       name, out, str(chunk), *extra], env=env))
-    for p in procs:
-        assert p.wait(timeout=600) == 0
-    return json.load(open(out))
+from gloo_runs import gloo_run
 
 
 @pytest.mark.parametrize("name,world,chunk", [("kip320_n2", 2, 97), ("asyncisr_v2", 2, 50), ("frl_tiny", 3, 7),
                                               ("kip320_n2", 1, 1000)])
 def test_sharded_bfs_matches_golden(name, world, chunk, tmp_path, goldens):
     g = goldens[name]
-    r = _run(name, world, chunk, tmp_path)
+    r = gloo_run(name, world, chunk, tmp_path)
     assert (r["distinct"], r["generated"], r["depth"], r["deadlocks"]) == (
         g["distinct"], g["generated"], g["depth"], g["deadlocks"])
     assert r["levels"] == g["levels"] and r["complete"] and r["violation"] is None
@@ -50,14 +21,14 @@ def test_sharded_bfs_matches_golden(name, world, chunk, tmp_path, goldens):
 
 def test_sharded_bfs_stops_on_violation(tmp_path, goldens):
     g = goldens["trunchw_n2"]
-    r = _run("trunchw_n2", 2, 200, tmp_path)
+    r = gloo_run("trunchw_n2", 2, 200, tmp_path)
     first = min(l for l in g["first_violation_level"].values() if l)
     assert r["violation"] is not None and not r["complete"]
     assert r["depth"] == first - 1                          # levels fully expanded before the violating one
     # the error trace is walked across ranks through the parent words: shortest, and a real behaviour
     assert r["violation"]["level"] == first and r["trace_len"] == first and r["trace_ok"] is True
     assert len(r["trace_ranks"]) == 2                       # it does hop between the two ranks' stores
-    r = _run("trunchw_n2", 2, 200, tmp_path, extra=("cont",))
+    r = gloo_run("trunchw_n2", 2, 200, tmp_path, extra=("cont",))
     assert (r["distinct"], r["generated"], r["depth"]) == (g["distinct"], g["generated"], g["depth"])
 
 
@@ -66,7 +37,7 @@ def test_device_sync_driver_loop_matches_golden(name, world, chunk, tmp_path, go
     """The driver's side of the device-synchronised protocol (one board per level, rounds without collectives of its
     own), over a stand-in whose rounds exchange through gloo: same counts and widths for any world size."""
     g = goldens[name]
-    r = _run(name, world, chunk, tmp_path, extra=("board",))
+    r = gloo_run(name, world, chunk, tmp_path, extra=("board",))
     assert (r["distinct"], r["generated"], r["depth"], r["deadlocks"]) == (
         g["distinct"], g["generated"], g["depth"], g["deadlocks"])
     assert r["levels"] == g["levels"] and r["complete"] and r["violation"] is None
@@ -76,8 +47,8 @@ def test_device_sync_driver_loop_matches_golden(name, world, chunk, tmp_path, go
 def test_device_sync_driver_loop_stops_on_violation(tmp_path, goldens):
     g = goldens["trunchw_n2"]
     first = min(l for l in g["first_violation_level"].values() if l)
-    r = _run("trunchw_n2", 2, 200, tmp_path, extra=("board",))
+    r = gloo_run("trunchw_n2", 2, 200, tmp_path, extra=("board",))
     assert r["violation"] is not None and not r["complete"] and r["depth"] == first - 1
     assert r["violation"]["level"] == first and r["trace_len"] == first and r["trace_ok"] is True
-    r = _run("trunchw_n2", 2, 200, tmp_path, extra=("board", "cont"))
+    r = gloo_run("trunchw_n2", 2, 200, tmp_path, extra=("board", "cont"))
     assert (r["distinct"], r["generated"], r["depth"], r["levels"]) == (g["distinct"], g["generated"], g["depth"], g["levels"])

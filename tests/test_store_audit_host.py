@@ -6,25 +6,17 @@ import os
 import numpy as np
 import pytest
 
-from conftest import REFERENCE, ROOT, needs_reference
+from conftest import ROOT, needs_reference
+from store_audit import AuditLib
 
 AUDITED = ["kip320_n2", "asyncisr_v2", "kip320sym_n2"]
 
 
-def _audit_lib(registry, name):
-    from hostmodel import lower_model
-    from store_audit import AuditLib
-    spec = registry[name]
-    m = lower_model(spec["module"], [REFERENCE, os.path.join(ROOT, "models")], open(os.path.join(ROOT, spec["cfg"])).read(),
-                    name=name)
-    return AuditLib(name, m.header, m.invariants_header)
-
-
 @pytest.fixture(scope="module")
-def clean_stores(registry):
+def clean_stores():
     out = {}
     for name in AUDITED:
-        a = _audit_lib(registry, name)
+        a = AuditLib.for_registered(name)
         out[name] = (a, a.host_bfs(sites=True))     # the order coverage.json was made in
     return out
 
@@ -105,11 +97,11 @@ def test_audit_rejects_a_corrupted_store(name, how, check, clean_stores, goldens
 
 
 @needs_reference
-def test_audit_finds_the_first_violating_level(registry, goldens):
+def test_audit_finds_the_first_violating_level(goldens):
     """trunchw_n2 violates its invariants: the violators the audit lists start at the golden's first violation level,
     and the counterexample build_trace's rule picks there is an invariant violation of that level."""
     from store_audit import expected_violation
-    a = _audit_lib(registry, "trunchw_n2")
+    a = AuditLib.for_registered("trunchw_n2")
     st = a.host_bfs()
     found = a.check_store(st["states"], st["parents"], st["widths"], st["n_expanded"], check_deadlock=False)
     first = min(l for l in goldens["trunchw_n2"]["first_violation_level"].values() if l)
@@ -120,9 +112,9 @@ def test_audit_finds_the_first_violating_level(registry, goldens):
 
 
 @needs_reference
-def test_audit_of_a_bounded_store(registry, goldens):
+def test_audit_of_a_bounded_store(goldens):
     """A store that stops after a level end (its last level not expanded) passes; so does closure, level by level."""
-    a = _audit_lib(registry, "kip320_n2")
+    a = AuditLib.for_registered("kip320_n2")
     st = a.host_bfs(stop_after=500)
     assert st["n_expanded"] == len(st["widths"]) - 1
     assert st["widths"] == goldens["kip320_n2"]["levels"][: len(st["widths"])]

@@ -9,6 +9,8 @@ are described in test_constraint_violations_host.py, which checks them against O
 checked against the goldens, its whole store and violator ring against the host audit (store_audit.audit_checker),
 and every state of its counterexample against Oracle A, transition by transition.
 """
+import functools
+import json
 import os
 import subprocess
 import sys
@@ -16,79 +18,32 @@ import sys
 import numpy as np
 import pytest
 
+import gpu_runs
 from conftest import ROOT
+from gpu_runs import CONSTRAINT_MODELS, compare_runs, fused_run, two_kernel_run
+from kafka_specification_b200 import build
+from oracle_a_actions import OracleA
 
 pytestmark = pytest.mark.gpu
 
-MODELS = ["minibound", "minibound_mixed", "minibound_init", "minibound_allout", "minibound_nodead", "minibound_sym",
-          "asyncisr_bounded"]
 DISCARDED_FIRST = {"minibound", "minibound_init", "asyncisr_bounded"}     # every first violator is a discarded state
+
+checker = functools.partial(gpu_runs.checker, table_log2=16)
+audited_run = functools.partial(gpu_runs.audited_run, table_log2=16)
 
 
 @pytest.fixture(scope="module")
 def coverage_golden():
-    import json
     with open(os.path.join(ROOT, "tests", "golden", "coverage.json")) as f:
         return json.load(f)
 
 
-@pytest.fixture(scope="module")
-def all_models():
-    """The registry build() compiles: these models are test-only, registered in tests/specs/MODELS.json."""
-    from kafka_specification_b200.build import registry
-    return registry()
-
-
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 16)
-    return Checker(name, **kw)
-
-
-class OracleA:
-    """Oracle A's interpreter for one registered model: initial states, labelled successors, predicates."""
-
-    def __init__(self, all_models, name):
-        import tla_interp
-        from kafka_specification_b200.build import tla_search_dirs
-        from kafka_specification_b200.frontend.cfg import parse_cfg
-        from kafka_specification_b200.frontend.modules import load_root
-        from oracle_a_actions import LabelledInterp
-        spec = all_models[name]
-        self.cfg = parse_cfg(open(os.path.join(ROOT, spec["cfg"])).read())
-        root = load_root(spec["module"], tla_search_dirs())
-        self.it = LabelledInterp(root, self.cfg)
-        init_e, self.next_e = tla_interp.resolve_init_next(root, self.cfg)
-        self.inits = self.it.init_states(init_e)
-
-    def text(self, st):
-        from kafka_specification_b200.frontend.values import fmt
-        return "\n".join(f"/\\ {v} = {fmt(st[v])}" for v in self.it.variables)
-
-    def holds(self, name, st):
-        return self.it.eval_named_predicate(name, st)
-
-    def violated(self, st):
-        return [inv for inv in self.cfg.invariants if not self.holds(inv, st)]
-
-    def in_model(self, st):
-        return all(self.holds(c, st) for c in self.cfg.constraints)
-
-
 def assert_trace_is_an_oracle_a_behaviour(oa, trace, violation):
-    """The first state is an initial state, each next one a successor of its predecessor under the action the trace
-    names, every state but the last is in the model and violates nothing, and the last one violates the reported
-    invariant.  Returns the Oracle A state of the last one."""
+    """The trace replays under Oracle A (OracleA.replay), every state but the last is in the model and violates
+    nothing, and the last one's first violated invariant is the reported one.  Returns the Oracle A state of the last
+    one."""
     assert len(trace) == violation["trace_len"] == violation["level"]
-    assert trace[0]["action"] is None
-    by_text = {oa.text(s): s for s in oa.inits}
-    assert trace[0]["text"] in by_text, "the first state is not an initial state"
-    states = [by_text[trace[0]["text"]]]
-    for i, t in enumerate(trace[1:], start=1):
-        nxt = [s1 for s1, label in oa.it.labelled_successors(oa.next_e, states[-1])
-               if label == t["action"]["name"] and oa.text(s1) == t["text"]]
-        assert nxt, f"trace state {i + 1} is not a {t['action']['name']} successor of state {i}:\n{t['text']}"
-        states.append(nxt[0])
+    states = oa.replay(trace)
     for i, st in enumerate(states[:-1]):
         assert oa.in_model(st) and not oa.violated(st), f"trace state {i + 1} of {len(states)} violates something"
     last = states[-1]
@@ -104,28 +59,12 @@ def first_violation(g):
     return lvl, {k for k, v in levels.items() if v == lvl}
 
 
-def audited_run(name, details=False, **opts):
-    """One kmc_run (the fused path), the audit of its store and violator ring, the run's trace and record; with
-    `details` also its coverage and the TLC text of every stored state."""
-    from store_audit import audit_checker
-    with checker(name, **opts) as ck:
-        r = ck.run()
-        # the initial states only (none when recovering): the successors are inserted by the expand kernel
-        assert r.stats["launches_insert"] == (0 if "recover" in opts else 1)
-        rep = audit_checker(ck, r.levels, r.distinct)
-        record = ck.violation_record() if r.violation else None
-        if details:
-            rep["coverage"] = ck.coverage()
-            rep["texts"] = [ck.decoder.text(row) for row in ck.copy_states(0, r.distinct)]
-    return r, rep, record
-
-
 @pytest.mark.parametrize("cont", [False, True])
-@pytest.mark.parametrize("name", MODELS)
-def test_fused_run_against_golden_audit_and_oracle_a(name, cont, all_models, goldens, coverage_golden):
+@pytest.mark.parametrize("name", CONSTRAINT_MODELS)
+def test_fused_run_against_golden_audit_and_oracle_a(name, cont, goldens, coverage_golden):
     from golden.make_golden import state_digest
     g = goldens[name]
-    r, rep, record = audited_run(name, details=True, cont=cont)
+    r, rep = audited_run(name, details=True, cont=cont)
     lvl, invs = first_violation(g)
     if cont or lvl is None:
         assert r.complete and r.queue == 0
@@ -136,7 +75,7 @@ def test_fused_run_against_golden_audit_and_oracle_a(name, cont, all_models, gol
         c, cov = coverage_golden[name], rep["coverage"]
         assert {a["name"]: a["generated"] for a in cov["actions"]} == c["per_action"]
         assert cov["init"]["generated"] == c["num_init"] and cov["complete"]
-        if not all_models[name].get("symmetry"):
+        if not build.registry()[name].get("symmetry"):
             assert cov["sites"] == c["per_site"]
             assert state_digest(rep["texts"]) == g["state_digest"]
     else:
@@ -150,18 +89,18 @@ def test_fused_run_against_golden_audit_and_oracle_a(name, cont, all_models, gol
     v = r.violation
     assert v["kind"] == "invariant" and v["level"] == lvl and v["invariant"] in invs and v["trace_len"] == lvl
     assert rep["violation"]["level_end"] == lvl - 1
-    oa = OracleA(all_models, name)
+    oa = OracleA(name)
     last = assert_trace_is_an_oracle_a_behaviour(oa, r.trace, v)
     if name in DISCARDED_FIRST:
         assert not oa.in_model(last) and not oa.holds("Bound", last)
     # the reported record is the trace's last state, with the parent word of the previous trace state
+    record = rep["record"]
     assert record[0] == r.trace[-1]["words"]
     if lvl > 1:
         assert (record[1] >> 56) == [a["name"] for a in registry_actions(name)].index(r.trace[-1]["action"]["name"])
 
 
 def registry_actions(name):
-    import json
     return json.load(open(os.path.join(ROOT, "build", "models", name, "model.json")))["actions"]
 
 
@@ -184,33 +123,27 @@ def test_every_initial_state_discarded_leaves_an_empty_store(goldens):
         assert cov["init"] == {**cov["init"], "distinct": 0, "generated": 3}
 
 
-@pytest.mark.parametrize("name,cont", [(n, c) for n in MODELS if n != "minibound_allout" for c in (False, True)])
+@pytest.mark.parametrize("name,cont", [(n, c) for n in CONSTRAINT_MODELS if n != "minibound_allout"
+                                       for c in (False, True)])
 def test_two_kernel_pipeline_reports_the_same_violation(name, cont):
     """kmc_shard_* at world 1 (expand -> candidate buffer -> k_insert): the same counts, widths and violation -- kind,
     invariant, level, trace length and fingerprint -- as the fused path."""
-    from test_fused_expand_insert import fused_run, two_kernel_run
-    (a, sets_a), (b, sets_b) = fused_run(name, cont=cont, table_log2=16), two_kernel_run(name, cont=cont, table_log2=16)
-    assert a["levels"] == b["levels"]
-    for k in ("distinct", "generated", "deadlocks", "out_of_model", "violation"):
-        assert a[k] == b[k], k
-    if name != "minibound_sym":       # under SYMMETRY the stored members depend on which insert won
-        assert a["sites"] == b["sites"]
-        for x, y in zip(sets_a, sets_b):
-            assert np.array_equal(x, y)
+    compare_runs(fused_run(name, cont=cont, table_log2=16), two_kernel_run(name, cont=cont, table_log2=16),
+                 symmetric=name == "minibound_sym")
 
 
 @pytest.mark.parametrize("cont,ring", [(False, 1 << 9), (True, 1 << 11)])
-def test_discarded_counterexample_through_spilled_levels(cont, ring, all_models, goldens):
+def test_discarded_counterexample_through_spilled_levels(cont, ring, goldens):
     """asyncisr_bounded (4,088 states) with a spilling ring: levels below the one being expanded live in host memory,
     so the trace of the level-6 violator (a discarded successor) walks from the ring into the spilled levels."""
     g = goldens["asyncisr_bounded"]
-    r, rep, _ = audited_run("asyncisr_bounded", cont=cont, spill=True, max_states=ring)
+    r, rep = audited_run("asyncisr_bounded", cont=cont, spill=True, max_states=ring)
     assert r.stats["max_states"] == ring < g["distinct"]
     if cont:
         assert r.complete and (r.distinct, r.levels, r.stats["out_of_model"]) == (g["distinct"], g["levels"], g["out_of_model"])
     assert r.violation["level"] == 6 and r.violation["invariant"] == "VersionInBound"
-    last = assert_trace_is_an_oracle_a_behaviour(OracleA(all_models, "asyncisr_bounded"), r.trace, r.violation)
-    assert not OracleA(all_models, "asyncisr_bounded").in_model(last)
+    last = assert_trace_is_an_oracle_a_behaviour(OracleA("asyncisr_bounded"), r.trace, r.violation)
+    assert not OracleA("asyncisr_bounded").in_model(last)
 
 
 @pytest.mark.parametrize("cont", [False, True])
@@ -225,7 +158,7 @@ def test_checkpoint_before_the_violating_level_and_recover(tmp_path, cont, golde
     assert not a.complete and a.violation is None and a.levels == g["levels"][:4]
     with checker("asyncisr_bounded", cont=cont) as ck:
         want = ck.run()
-    r, rep, _ = audited_run("asyncisr_bounded", recover=d, cont=cont)
+    r, rep = audited_run("asyncisr_bounded", recover=d, cont=cont)
     assert r.stats["out_of_model"] == want.stats["out_of_model"] == rep["found"]["out_of_model"]
     assert 0 < a.stats["out_of_model"] < r.stats["out_of_model"]
     if cont:
@@ -249,19 +182,18 @@ def test_cli_reports_a_discarded_violator():
     assert ":> 3" in last.split("\n\n")[0], last
 
 
-def test_symmetry_counterexample_is_the_rule_pick_over_orbits(all_models):
+def test_symmetry_counterexample_is_the_rule_pick_over_orbits():
     """minibound_sym: OneFull is first violated at level 3 by three orbits, reached only through members that are not
     their canonical form.  The reported counterexample is the rule's pick over orbits -- deadlocks first, then the
     smallest fingerprint of the canonical form -- computed on the host from the lowered model's own BFS, whichever
     member the GPU stored; and two runs report the same orbit."""
-    from store_audit import AuditLib, fingerprint
-    from test_constraint_violations_host import _host_audit, expected_orbit
+    from store_audit import AuditLib, expected_orbit, fingerprint, host_audit
     a = AuditLib.for_built_model("minibound_sym")
-    _, _, found = _host_audit(all_models, "minibound_sym")
+    _, _, found = host_audit("minibound_sym")
     orbit, fp = expected_orbit(a, found)
     got = []
     for _ in range(2):
-        r, rep, record = audited_run("minibound_sym")
+        r, _ = audited_run("minibound_sym")
         v = r.violation
         assert (v["kind"], v["invariant"], v["level"]) == ("invariant", "OneFull", 3)
         words = np.asarray([r.trace[-1]["words"]], dtype=np.uint64)

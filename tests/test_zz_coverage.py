@@ -4,6 +4,7 @@ CPU: the lowering's site -> action map, the committed coverage goldens, the labe
 harness, the CLI's report format.  GPU: every parity model's counts against the goldens, the sums, the parent
 words, stopped / recovered / multi-GPU runs, and the CLI end to end.
 """
+import functools
 import json
 import os
 import re
@@ -14,11 +15,12 @@ from collections import Counter
 import numpy as np
 import pytest
 
+import gpu_runs
 from conftest import ROOT, needs_reference
-from test_gpu_parity import ALL_MODELS
+from gpu_runs import ALL_MODELS
+from store_audit import NO_PARENT, copy_parents
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-NO_PARENT = 0x0000FFFFFFFFFFFF
 
 
 @pytest.fixture(scope="module")
@@ -40,11 +42,10 @@ def by_action(per_site, site_action, names):
 def test_every_model_lowers_with_site_actions_matching_the_emit_labels(registry):
     """SITE_ACTION[i] is the label of site i's sink.emit, model.json agrees with the header, and the digest that
     checkpoints are checked against is the one the models had before coverage existed."""
-    from kafka_specification_b200.build import tla_search_dirs
-    from kafka_specification_b200.lower.model import lower_model
+    from hostmodel import lower_registered
     digests = json.load(open(os.path.join(GOLDEN, "body_digests.json")))
-    for name, spec in registry.items():
-        m = lower_model(spec["module"], tla_search_dirs(), open(os.path.join(ROOT, spec["cfg"])).read(), name=name)
+    for name in registry:
+        m = lower_registered(name)
         assert m.digest == digests[name], name
         n = int(re.search(r"static constexpr int NUM_SITES = (\d+);", m.header).group(1))
         table = re.search(r"SITE_ACTION\[[^\]]*\] = \{([^}]*)\};", m.header).group(1)
@@ -63,9 +64,8 @@ def test_every_model_lowers_with_site_actions_matching_the_emit_labels(registry)
 
 @needs_reference
 def test_init_span_is_the_initial_predicate():
-    from kafka_specification_b200.build import tla_search_dirs
-    from kafka_specification_b200.lower.model import lower_model
-    m = lower_model("MiniLock", tla_search_dirs(), open(os.path.join(ROOT, "tests", "specs", "MiniLock.cfg")).read())
+    from hostmodel import lower_registered
+    m = lower_registered("minilock")
     src = open(os.path.join(ROOT, "tests", "specs", "MiniLock.tla")).read().split("\n")
     assert m.init["name"] == "Init" and m.init["module"] == "MiniLock"
     assert src[m.init["line"] - 1][m.init["col"] - 1:].startswith("Init")
@@ -77,13 +77,12 @@ def test_oracle_a_action_labels_agree_with_the_lowering(name, registry, goldens)
     """TLC's rule (first operator below Next), applied by Oracle A to the .tla text, gives the same generated count
     per action as the lowered model's emit labels on the host."""
     from kafka_specification_b200.build import tla_search_dirs
-    from kafka_specification_b200.lower.model import lower_model
-    from hostmodel import run_host
+    from hostmodel import lower_registered, run_host
     from oracle_a_actions import run_bfs_by_action
     spec = registry[name]
     cfg_text = open(os.path.join(ROOT, spec["cfg"])).read()
     a = run_bfs_by_action(spec["module"], tla_search_dirs(), cfg_text)
-    h = run_host(lower_model(spec["module"], tla_search_dirs(), cfg_text, name=name))
+    h = run_host(lower_registered(name))
     assert a["generated"] == h["generated"] == goldens[name]["generated"]
     assert {k: v for k, v in h["per_action"].items() if v} == a["per_action"]
 
@@ -145,16 +144,11 @@ def test_cli_coverage_report_format(capsys):
 
 
 # ---------------------------------------------------------------------------------------------------------- GPU
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 24)
-    return Checker(name, **kw)
+checker = functools.partial(gpu_runs.checker, table_log2=24)
 
 
 def parents_histogram(ck, distinct):
-    par = np.empty(distinct, dtype=np.uint64)
-    if distinct:
-        assert ck.lib.kmc_copy_parents(ck.ctx, 0, distinct, par.ctypes.data) == 0
+    par = copy_parents(ck, 0, distinct)
     init = (par & np.uint64(NO_PARENT)) == np.uint64(NO_PARENT)
     acts = (par[~init] >> np.uint64(56)).astype(np.int64)
     names = [a["name"] for a in ck.meta["actions"]]

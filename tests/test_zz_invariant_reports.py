@@ -6,10 +6,11 @@ import sys
 
 import pytest
 
+import gpu_runs
 from conftest import ROOT
+from gpu_runs import assert_oracle_b_trace, report_summary as summary
 from hostmodel import HostModel
-from test_gpu_parity import _assert_trace_is_behaviour
-from test_zz_constraint_violations import OracleA
+from oracle_a_actions import OracleA
 
 pytestmark = pytest.mark.gpu
 
@@ -19,57 +20,32 @@ MINI = ["minibound", "minibound_mixed", "minibound_init", "minibound_sym", "asyn
 RING = 1 << 16
 
 
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 24 if name.endswith("_n2") or name.startswith("mini") or name == "asyncisr_bounded" else 0)
-    if not kw["table_log2"]:
-        del kw["table_log2"]
-    return Checker(name, **kw)
-
-
-def summary(reports, words=True):
-    """What a run reports per invariant.  (The states before the last one are not part of it: a state's parent is the
-    generator whose insert won, which may differ from run to run, as for kmc_violation's trace; under SYMMETRY
-    neither is the last one: the pick is an orbit, and the member stored is the one whose insert won.)"""
-    return [(r["invariant"], r["level"], r["violators_first_level"], r["violators"], r["fingerprint"], r["trace_len"],
-             r["trace"][-1]["words"] if r["trace"] and words else None) for r in reports]
+def checker(name, **opts):
+    """A set of 2^24 slots for the small models, the engine's default size for the others."""
+    if name.endswith("_n2") or name.startswith("mini") or name == "asyncisr_bounded":
+        opts.setdefault("table_log2", 24)
+    return gpu_runs.checker(name, **opts)
 
 
 def assert_kafka_trace(name, ck, rep):
-    """Oracle B checks every step (as _assert_trace_is_behaviour); only the reported invariant must hold on the earlier
-    states and fail on the last one."""
+    """Oracle B checks every step; only the reported invariant must hold on the earlier states and fail on the last
+    one."""
     import kso
-    saved = ck.meta["invariants"]
-    ck.meta["invariants"] = [rep["invariant"]]
-    try:
-        if rep["invariant"] in kso.INVARIANTS:
-            _assert_trace_is_behaviour(name, rep["trace"], ck)
-    finally:
-        ck.meta["invariants"] = saved
+    if rep["invariant"] in kso.INVARIANTS:
+        assert_oracle_b_trace(name, rep["trace"], ck.decoder, [rep["invariant"]])
 
 
 def assert_mini_trace(oa, rep):
-    assert rep["trace"][0]["action"] is None
-    by_text = {oa.text(s): s for s in oa.inits}
-    states = [by_text[rep["trace"][0]["text"]]]
-    for i, t in enumerate(rep["trace"][1:], start=1):
-        nxt = [s1 for s1, label in oa.it.labelled_successors(oa.next_e, states[-1])
-               if label == t["action"]["name"] and oa.text(s1) == t["text"]]
-        assert nxt, f"trace state {i + 1} is not a {t['action']['name']} successor of state {i}"
-        states.append(nxt[0])
+    """The trace replays under Oracle A (OracleA.replay); every state but the last is in the model and satisfies the
+    reported invariant, and the last one violates it."""
+    states = oa.replay(rep["trace"])
     for st in states[:-1]:
         assert oa.in_model(st) and oa.holds(rep["invariant"], st)
     assert not oa.holds(rep["invariant"], states[-1])
 
 
-@pytest.fixture(scope="module")
-def all_models():
-    from kafka_specification_b200.build import registry
-    return registry()
-
-
 @pytest.mark.parametrize("name", KAFKA + MINI + ["leaderinisr_init"])
-def test_every_violated_invariant_is_reported(name, goldens, all_models):
+def test_every_violated_invariant_is_reported(name, goldens):
     g = goldens[name]
     want = {i: l for i, l in g["first_violation_level"].items() if l is not None}
     with checker(name, cont=True) as ck:
@@ -97,7 +73,7 @@ def test_every_violated_invariant_is_reported(name, goldens, all_models):
             if name in KAFKA:
                 assert_kafka_trace(name, ck, x)
         if name in MINI:
-            oa = OracleA(all_models, name)
+            oa = OracleA(name)
             for x in reps:
                 assert_mini_trace(oa, x)
         words = name != "minibound_sym"
@@ -113,33 +89,11 @@ def test_without_continue_nothing_is_collected():
         assert ck.invariant_reports() == []
 
 
-def _shard_run(name, **opts):
-    """The two-kernel kmc_shard_* path at world 1 (expand into the candidate buffer, k_insert, level end)."""
-    import numpy as np
-    from kafka_specification_b200.runtime import Checker
-    with Checker(name, cont=True, **opts) as ck:
-        lib, c = ck.lib, ck.ctx
-        assert lib.kmc_shard_begin(c) == 0 and lib.kmc_shard_seed_init(c) == 0
-        from kafka_specification_b200.runtime import ShardBuffers
-        import ctypes
-        b = ShardBuffers()
-        assert lib.kmc_shard_buffers(c, ctypes.byref(b)) == 0
-        tail, first, count = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
-        counts = np.zeros(8, dtype=np.uint64)
-        assert lib.kmc_shard_counts(c, counts.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64))) == 0
-        assert lib.kmc_shard_insert(c, b.recv, int(counts[0]), ctypes.byref(tail)) == 0
-        assert lib.kmc_shard_level_done(c, ctypes.byref(first), ctypes.byref(count)) == 0
-        chunk = max(1, b.region_rows // 32)
-        while count.value:
-            f, n = first.value, count.value
-            for off in range(0, n, chunk):
-                k = min(chunk, n - off)
-                assert lib.kmc_shard_reset_cand(c) == 0
-                assert lib.kmc_shard_expand(c, f + off, k) == 0
-                assert lib.kmc_shard_counts(c, counts.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64))) == 0
-                assert lib.kmc_shard_insert(c, b.recv, int(counts[0]), ctypes.byref(tail)) == 0
-            assert lib.kmc_shard_level_done(c, ctypes.byref(first), ctypes.byref(count)) == 0
-        assert lib.kmc_shard_sync(c) == 0
+def shard_path_reports(name):
+    """The reports of the two-kernel kmc_shard_* path at world 1 (gpu_runs.shard_levels)."""
+    with checker(name, cont=True) as ck:
+        gpu_runs.shard_levels(ck, cont=True)
+        ck._check(ck.lib.kmc_shard_sync(ck.ctx))
         return summary(ck.invariant_reports())
 
 
@@ -147,8 +101,7 @@ def _shard_run(name, **opts):
 def test_shard_path_at_world_1_reports_the_same(name):
     with checker(name, cont=True) as ck:
         fused = summary(ck.run().invariant_violations)
-    tl = {"table_log2": 24} if not name.startswith("first") else {}
-    assert _shard_run(name, **tl) == fused
+    assert shard_path_reports(name) == fused
 
 
 def test_spill_and_a_small_ring_report_the_same():

@@ -2,15 +2,16 @@
 agree with Oracle A / Oracle B on the host, tests/test_generic_frontend.py and the goldens' `sources`) and no GPU
 verdict yet.  The file name and tests/conftest.py make them run LAST, so that -x cannot let them hide the
 verdicts of the parity tests proper."""
+import functools
+
 import pytest
+
+import gpu_runs
+from gpu_runs import VIOLATING_MODELS
 
 pytestmark = pytest.mark.gpu
 
-
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 24)
-    return Checker(name, **kw)
+checker = functools.partial(gpu_runs.checker, table_log2=24)
 
 
 @pytest.mark.parametrize("name", ["miniqueue", "minimsgs", "miniwindow"])
@@ -43,7 +44,7 @@ def test_zz_protocol_variants_at_headline_bounds(name, goldens):
     assert r.violation is not None and r.violation["kind"] == "invariant" and r.violation["level"] == first
 
 
-@pytest.mark.parametrize("name", ["trunchw_small", "kip101_small", "kip279_small", "firsttry_small", "kip320_with279_small"])
+@pytest.mark.parametrize("name", VIOLATING_MODELS)
 def test_zz_three_replica_state_sets_match_oracle_a(name, goldens):
     """The 3-replica models whose StrongIsr violations the reference describes: the whole reachable state set
     (1.4..2.0e6 states), decoded to TLC text, against the digest Oracle A -- the interpreter of the unchanged .tla

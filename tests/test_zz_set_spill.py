@@ -15,15 +15,11 @@ import numpy as np
 import pytest
 
 from conftest import REFERENCE, ROOT, needs_reference
+from gpu_runs import audited_run, checker, report_summary
 
 pytestmark = pytest.mark.gpu
 
 BADARG, STORE_FULL = -1, -5
-
-
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    return Checker(name, **kw)
 
 
 def max_fanout(name):
@@ -33,10 +29,7 @@ def max_fanout(name):
 
 def spill_run(name, table_log2, max_states, **opts):
     """One set_spill run and the audit of its store; returns (RunResult, audit report)."""
-    from store_audit import audit_checker
-    with checker(name, set_spill=True, table_log2=table_log2, max_states=max_states, **opts) as ck:
-        r = ck.run()
-        rep = audit_checker(ck, r.levels, r.distinct)
+    r, rep = audited_run(name, set_spill=True, table_log2=table_log2, max_states=max_states, **opts)
     st = r.stats
     # each key reaches host memory once, and what is left in the table stays below its load limit
     assert st["set_host_keys"] <= r.distinct and r.distinct - st["set_host_keys"] <= st["table_slots"] // 2
@@ -66,11 +59,6 @@ def test_golden_and_audit_through_many_flushes(name, table_log2, slot_bytes, gol
     assert st["set_filtered"] > 0 and st["gpu_ms_set_spill"] > 0
 
 
-def _summary(reports):
-    return [(x["invariant"], x["level"], x["violators_first_level"], x["violators"], x["fingerprint"], x["trace_len"],
-             x["trace"][-1]["words"]) for x in reports]
-
-
 # the stopped runs hold ~34,000 states: a 2^12-slot table; the complete ones ~2 million: 2^15
 @pytest.mark.parametrize("cont,table_log2", [(False, 12), (True, 15)])
 @pytest.mark.parametrize("name", ["trunchw_small", "firsttry_small"])
@@ -86,7 +74,7 @@ def test_violations_are_those_of_a_default_run(name, cont, table_log2, goldens):
            (w["kind"], w["invariant"], w["level"], w["trace_len"], w["fingerprint"])
     assert r.trace[-1]["words"] == want.trace[-1]["words"]
     assert rep["violation"]["fingerprint"] == v["fingerprint"] and rep["violation"]["level"] == v["level"]
-    assert _summary(r.invariant_violations) == _summary(want.invariant_violations)
+    assert report_summary(r.invariant_violations) == report_summary(want.invariant_violations)
     if cont:
         assert_golden(r, g)
 
@@ -102,7 +90,7 @@ def test_constraint_discarded_violators(cont, goldens):
     r, rep = spill_run("asyncisr_bounded", table_log2, g["distinct"] + 4096, cont=cont)
     assert r.violation == want.violation and r.violation["level"] == 6
     assert r.stats["out_of_model"] == want.stats["out_of_model"] == rep["found"]["out_of_model"]
-    assert _summary(r.invariant_violations) == _summary(want.invariant_violations)
+    assert report_summary(r.invariant_violations) == report_summary(want.invariant_violations)
     if cont:
         assert_golden(r, g)
         assert r.stats["out_of_model"] == g["out_of_model"] and r.stats["set_flushes"] >= 10

@@ -9,6 +9,7 @@ every violator the engine records.
 
 Also here: the fingerprint set alone (kmc_fpset_*) with 8-byte and 16-byte slots, at the edges of its probe sequence.
 """
+import functools
 import json
 import os
 import subprocess
@@ -17,30 +18,16 @@ import sys
 import numpy as np
 import pytest
 
+import gpu_runs
 from conftest import ROOT
-from test_gpu_parity import ALL_MODELS
+from gpu_runs import ALL_MODELS, VIOLATING_MODELS
 
 pytestmark = pytest.mark.gpu
 
 CHECKPOINT = os.path.join(ROOT, "tests", "golden", "checkpoint_kip320_n2")
 
-
-def checker(name, **kw):
-    from kafka_specification_b200.runtime import Checker
-    kw.setdefault("table_log2", 22)
-    return Checker(name, **kw)
-
-
-def audit_run(name, check_deadlock=None, **opts):
-    """One kmc_run, then the audit of its whole store; returns (RunResult, audit report)."""
-    from store_audit import audit_checker
-    if check_deadlock is not None:
-        opts["check_deadlock"] = check_deadlock
-    with checker(name, **opts) as ck:
-        r = ck.run()
-        rep = audit_checker(ck, r.levels, r.distinct, check_deadlock=check_deadlock)
-    assert sum(rep["widths"]) == r.distinct
-    return r, rep
+checker = functools.partial(gpu_runs.checker, table_log2=22)
+audit_run = functools.partial(gpu_runs.audited_run, table_log2=22)
 
 
 @pytest.mark.parametrize("name", ALL_MODELS)
@@ -50,7 +37,7 @@ def test_store_audit_full_run(name, goldens):
     assert r.complete and rep["widths"] == g["levels"] and rep["found"]["generated"] == g["generated"]
 
 
-@pytest.mark.parametrize("name", ["trunchw_small", "kip101_small", "kip279_small", "firsttry_small", "kip320_with279_small"])
+@pytest.mark.parametrize("name", VIOLATING_MODELS)
 def test_store_audit_stop_at_first_violation(name, goldens):
     r, rep = audit_run(name)
     first = min(l for l in goldens[name]["first_violation_level"].values() if l)
