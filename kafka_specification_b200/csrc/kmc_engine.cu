@@ -697,6 +697,9 @@ static constexpr int STAGE_BYTES = NWARPS * STAGE_ROWS * ROW * 8;
 static constexpr int FIXED_SMEM_BYTES = STAGE_BYTES + LIST_CAP * 2 + (4 * MAX_GROUP_SITES + NWARPS + 8) * 4;
 static constexpr int SPT_FIT = (227 * 1024 - 1024 - FIXED_SMEM_BYTES) / (EXPAND_BLOCK * W * 8);
 static constexpr int SPT = SPT_FIT > 4 ? 4 : SPT_FIT;
+// The widest state is 7 words: at W = 8 the warps' stage rows (32 x 64 rows of 9 words, 144 KB) and a tile of one state
+// per thread (1024 x 8 words, 64 KB) exceed the 226 KB of shared memory a CTA can have.  The lowering refuses wider
+// models with a message (lower/model.py, MAX_WORDS); W = 5, 6, 7 get SPT = 2, 1, 1.
 static_assert(SPT >= 1, "state too wide for the expand kernel's shared-memory tile");
 static constexpr int TILE = EXPAND_BLOCK * SPT;
 static_assert(TILE <= LIST_CAP, "a site's segment (<= TILE pairs) must fit one scatter round");

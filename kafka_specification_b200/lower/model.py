@@ -23,6 +23,7 @@ from .svals import LowerError, SLazy, is_atom_const, is_const, is_int_const
 
 LOWERING_VERSION = 3
 MAX_MASK_INVARIANTS = 64       # violated_invariants() returns one bit per INVARIANT
+MAX_WORDS = 7                  # widest packed state the expand kernel's shared-memory tile holds (kmc_engine.cu, SPT)
 
 
 @dataclass
@@ -551,6 +552,9 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
             apply_prefix(ty, *cfg.prefix[v])
         lay.add_variable(v, ty)
     lay.finish()
+    if lay.words > MAX_WORDS:
+        raise LowerError(f"the state packs into {lay.words} 64-bit words ({lay.bits} bits); the expand kernel "
+                         f"takes at most {MAX_WORDS} words")
     lw.layout = lay
 
     init_e, next_e = _resolve_init_next(lw)

@@ -43,7 +43,28 @@ def closed_form(module, cfg):
     if module == "FiniteReplicatedLog":
         nrep, L, R = len(c["Replicas"]), c["LogSize"], len(c["LogRecords"])
         return {"distinct": sum(R ** e for e in range(L + 1)) ** nrep, "depth": nrep * L + 1}
+    if module == "MiniWide" and c["Max"] == 1 and not cfg.symmetry:
+        return miniwide_closed_form(len(c["Procs"]) * c["Slots"], c["Budget"], c["Limit"], cfg.invariants)
     return {}
+
+
+def miniwide_closed_form(n, budget, limit, invariants):
+    """MiniWide with Max = 1 over n cells: a state is its set of full cells, one more per step, so level i + 1 holds the
+    C(n, i) states with i full cells, up to the Budget of the CONSTRAINT.  Each state with i full cells generates n - i
+    successors; those of the last level all have Budget + 1 full cells and are discarded (and no deadlock).  FewFull
+    (fewer than Limit full cells, Limit <= Budget) is first violated at level Limit + 1 by C(n, Limit) states, and
+    violated by every later state and every discarded successor."""
+    from math import comb
+    b = min(budget, n)
+    assert limit <= b, "the closed form covers a Limit the stored states reach"
+    levels = [comb(n, i) for i in range(b + 1)]
+    out = comb(n, b) * (n - b)
+    return {"distinct": sum(levels), "levels": levels, "depth": b + 1,
+            "generated": 1 + sum(comb(n, i) * (n - i) for i in range(b + 1)),
+            "deadlocks": 1 if b == n else 0, "out_of_model": out,
+            "first_violation_level": {inv: limit + 1 if inv == "FewFull" else None for inv in invariants},
+            "violators_first_level": {"FewFull": comb(n, limit)},
+            "violating_states": {inv: sum(levels[limit:]) + out if inv == "FewFull" else 0 for inv in invariants}}
 
 
 def main():
@@ -74,11 +95,6 @@ def main():
              "distinct": b["distinct"], "generated": b["generated"], "depth": b["depth"], "levels": b["levels"],
              "deadlocks": b["deadlocks"], "first_violation_level": b["first_violation_level"],
              "check_deadlock": cfg.check_deadlock, "sources": src}
-        cf = closed_form(spec["module"], cfg)
-        for k, v in cf.items():
-            assert g[k] == v, (name, k, g[k], v)
-        if cf:
-            g["sources"].append("closed_form")
         if spec.get("oracle_a"):
             # full-space statistics: never stop at a violation, deadlock checking off
             stats_cfg = cfg_text + "\nCHECK_DEADLOCK FALSE\n"
@@ -92,6 +108,14 @@ def main():
             if not spec.get("symmetry"):       # under SYMMETRY the choice of orbit representatives is free
                 g["state_digest"] = state_digest(a["states"])
             g["sources"].append("oracle_a")
+        cf = closed_form(spec["module"], cfg)
+        for k, v in cf.items():
+            if k in g:
+                assert g[k] == v, (name, k, g[k], v)
+        if cf and spec.get("oracle_a") and "violating_states" in cf:
+            assert a["violating_states"] == cf["violating_states"], (name, a["violating_states"])
+        if cf:
+            g["sources"].append("closed_form")
         out[name] = g
         print(f"{name}: distinct={g['distinct']} generated={g['generated']} depth={g['depth']} "
               f"viol={g['first_violation_level']} sources={g['sources']} ({time.time() - t0:.1f}s)", flush=True)
