@@ -109,12 +109,10 @@ extern "C" int kmc_cpu_bfs(uint64_t* st, int threads, int table_log2, uint64_t s
   bool complete = true;
 
   auto t0 = std::chrono::steady_clock::now();
-  // initial states (sequential, tiny)
-  for (int i = 0; i < M::NUM_INIT; ++i) {
-    State s;
-    memcpy(s.w, M::INIT_STATES[i], sizeof(s.w));
+  // initial states (sequential): the table, or every solution of the device form of Init
+  auto seed = [&](const State& s) {
     ws[0].generated++;
-    if (M::NUM_CONSTRAINTS && !M::in_model(s)) { ws[0].out_of_model++; continue; }
+    if (M::NUM_CONSTRAINTS && !M::in_model(s)) { ws[0].out_of_model++; return; }
     State c;
     M::canonicalize(s, c);
     if (table.put(fingerprint(c)) == 1) {
@@ -122,7 +120,22 @@ extern "C" int kmc_cpu_bfs(uint64_t* st, int threads, int table_log2, uint64_t s
       int inv = M::first_violated_invariant(s);
       if (inv >= 0 && inv < 16) ws[0].viol[inv]++;
     }
+  };
+#ifdef KMC_HAS_DEVICE_INIT
+  for (int b = 0; b < M::INIT_BRANCHES; ++b)
+    for (uint64_t i = 0; i < M::INIT_SPACE[b]; ++i) {
+      State s;
+      unsigned fail = 0;
+      if (M::init_candidate(b, i, s, fail)) seed(s);
+      if (fail) { st[4] = KMC_FAIL_LAYOUT; free(table.slots); return 1; }
+    }
+#else
+  for (int i = 0; i < M::NUM_INIT; ++i) {
+    State s;
+    memcpy(s.w, M::INIT_STATES[i], sizeof(s.w));
+    seed(s);
   }
+#endif
   distinct = frontier.size();
 
   auto on_level_end = [&]() noexcept {

@@ -14,8 +14,14 @@
  *   kmc_run             tlc2.tool.ModelChecker.doInit + runTLC: N x tlc2.tool.Worker.run --
  *                       the hot loop: StateQueue.sDequeue -> Tool.getNextStates ->
  *                       TLCState.fingerPrint -> FPSet.put -> Tool.isValid -> sEnqueue
+ *                       Level 1 comes from the lowered model's table of initial states or, for a
+ *                       model lowered with the device form of Init (model.json init.device), from
+ *                       k_init, which decodes every candidate assignment of Init's generators on the
+ *                       GPU and keeps those that satisfy the rest of Init (one GPU only: "gpus" > 1,
+ *                       world > 1 and the kmc_shard_* calls give KMC_E_BADARG)
  *   kmc_stats           ModelChecker.reportSuccess / printSummary ("N states generated,
- *                       M distinct states found, Q states left on queue", depth)
+ *                       M distinct states found, Q states left on queue", depth); init_generated
+ *                       and init_candidates count TLC's doInit ("N distinct states generated")
  *   kmc_violation       ModelChecker.doNext's invariant/deadlock failure report
  *   kmc_invariant_*     the same per invariant under -continue (first level, violators, counterexample)
  *   kmc_coverage        ModelChecker's coverage report (TLC -coverage: "distinct:generated" per action, at the
@@ -87,6 +93,9 @@ typedef struct {
   uint64_t set_filtered;    /* "set_spill": appended states removed because their key was in host memory */
   double gpu_ms_set_spill;  /* "set_spill": CUDA-event time of the flushes and filters (part of gpu_ms_total) */
   uint64_t set_link_bytes;  /* "set_spill": key bytes the flushes (device to host) and filters (host to device) moved */
+  uint64_t init_generated;  /* Init solutions, duplicates included (part of `generated`): NUM_INIT for a table model */
+  uint64_t init_candidates; /* device Init: candidate assignments k_init decoded; 0 for a table model */
+  double gpu_ms_init;       /* device Init: CUDA-event time of the k_init launches (part of gpu_ms_total) */
 } kmc_stats_t;
 
 typedef struct {
@@ -119,6 +128,7 @@ typedef struct {
   int32_t exact;            /* 1: the set key is a bijection of the state (<= 63 bits, or two words stored as a 128-bit key) */
   char name[128];
   char digest[32];
+  uint64_t init_candidates;  /* device Init: candidate assignments over all branches (num_init is then 0); 0 for a table */
 } kmc_model_info_t;
 
 /* model_lib: path of a lowered-model library (libkmc_<model>.so, built ahead of time by

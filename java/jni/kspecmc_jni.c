@@ -40,10 +40,11 @@ JNIEXPORT jint JNICALL Java_tlc2_gpu_Native_run(JNIEnv* env, jclass cls, jlong c
 JNIEXPORT jlongArray JNICALL Java_tlc2_gpu_Native_stats(JNIEnv* env, jclass cls, jlong ctx) {
   kmc_stats_t s;
   if (kmc_stats((kmc_ctx*)(intptr_t)ctx, &s) != KMC_OK) return NULL;
-  jlong v[9] = {(jlong)s.distinct, (jlong)s.generated, (jlong)s.queue, (jlong)s.depth, (jlong)s.deadlocks,
-                (jlong)s.out_of_model, (jlong)s.probes, (jlong)s.levels, (jlong)s.complete};
-  jlongArray a = (*env)->NewLongArray(env, 9);
-  (*env)->SetLongArrayRegion(env, a, 0, 9, v);
+  jlong v[11] = {(jlong)s.distinct, (jlong)s.generated, (jlong)s.queue, (jlong)s.depth, (jlong)s.deadlocks,
+                 (jlong)s.out_of_model, (jlong)s.probes, (jlong)s.levels, (jlong)s.complete,
+                 (jlong)s.init_generated, (jlong)s.init_candidates};
+  jlongArray a = (*env)->NewLongArray(env, 11);
+  (*env)->SetLongArrayRegion(env, a, 0, 11, v);
   return a;
 }
 

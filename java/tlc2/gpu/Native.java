@@ -24,7 +24,8 @@ public final class Native {
     /** kmc_run: blocking full BFS; returns the KMC_* status code. */
     public static native int run(long ctx);
 
-    /** kmc_stats: {distinct, generated, queue, depth, deadlocks, outOfModel, probes, levels, complete}. */
+    /** kmc_stats: {distinct, generated, queue, depth, deadlocks, outOfModel, probes, levels, complete, initGenerated,
+     *  initCandidates}. */
     public static native long[] stats(long ctx);
 
     /** kmc_violation: {kind, invariantIndex, level, traceLength, fingerprint} or null when kind == 0. */

@@ -1,6 +1,6 @@
 """Ahead-of-time build: ``.tla`` + ``.cfg``  ->  lowered header  ->  ``libkmc_<model>.so`` (sm_90a).
 
-    python -m kafka_specification_b200.build --all            # every model in models/ and tests/specs/MODELS.json
+    python -m kafka_specification_b200.build --all            # every model in models/ and tests/specs/MODELS*.json
     python -m kafka_specification_b200.build Kip320 models/Kip320.cfg --name kip320
 
 Artifacts go to ``build/`` (git-ignored):
@@ -182,12 +182,29 @@ def registry() -> dict:
     return {**reg, **test_models}
 
 
+DEVICE_INIT_REGISTRY = os.path.join(TEST_SPECS_DIR, "MODELS_device_init.json")
+
+
+def device_init_registry() -> dict:
+    """The models that test the device form of Init (tests/specs/MODELS_device_init.json): build_all() compiles them
+    too.  They are kept out of registry(), whose every header is pinned in tests/golden/header_digests.json; theirs
+    are pinned in tests/golden/device_init_header_digests.json."""
+    if not os.path.exists(DEVICE_INIT_REGISTRY):
+        return {}
+    with open(DEVICE_INIT_REGISTRY) as f:
+        models = json.load(f)
+    clash = set(registry()) & set(models)
+    if clash:
+        raise RuntimeError(f"models registered twice: {sorted(clash)}")
+    return models
+
+
 def build_all(force: bool = False, only: list[str] | None = None, verbose: bool = True, jobs: int = 0) -> dict[str, str]:
     """Lower (sequentially, it is fast) and compile (in parallel: nvcc dominates) every registered model."""
     from concurrent.futures import ThreadPoolExecutor
     build_dispatcher(force)
     todo = []
-    for name, spec in registry().items():
+    for name, spec in {**registry(), **device_init_registry()}.items():
         if only and name not in only:
             continue
         module, cfg_path = spec["module"], os.path.join(ROOT, spec["cfg"])

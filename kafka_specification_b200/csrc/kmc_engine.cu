@@ -184,6 +184,9 @@ struct DevCounters {
   unsigned long long inv_viol_seen;      // viol_count at the last level end (host-written)
   unsigned long long inv_count[64];      // violators per invariant over the run
   unsigned long long set_count;          // set_spill: keys a flush range copied out, or states a filter piece kept
+  // device Init (k_init): the candidates decoded and the solutions among them (also counted in `generated`)
+  unsigned long long init_candidates;
+  unsigned long long init_generated;
 };
 
 // Violating states are rare and terminal, so they go to a small ring: W state words, the
@@ -1040,6 +1043,88 @@ __global__ void __launch_bounds__(256) k_insert(Params p, const uint64_t* rows, 
   }
 }
 
+#ifdef KMC_HAS_DEVICE_INIT
+// ----------------------------------------------------------------------------------------
+// K0: device Init.  One candidate index of one branch per thread, grid-stride with 64-bit indices: the lowered
+// init_candidate() decodes it, runs the branch's filters and packs a solution.  A warp ballot compacts the solutions
+// into the warp's shared-memory stage (the rows of k_expand's stage, parent word NO_PARENT), which the warp inserts
+// through insert_stage whenever it holds STAGE_FLUSH rows or more.  Solutions, candidates, probes and out-of-model
+// initial states are counted per CTA in shared memory and flushed with one global atomic each.
+// ----------------------------------------------------------------------------------------
+static constexpr int INIT_BLOCK = 256;
+static constexpr int INIT_WARPS = INIT_BLOCK / 32;
+static constexpr int CTA_INIT_GEN = CTA_ACTION + M::NUM_ACTIONS, CTA_INIT_CAND = CTA_INIT_GEN + 1;
+
+__global__ void __launch_bounds__(INIT_BLOCK) k_init(Params p, int branch, uint64_t first, uint64_t count) {
+  __shared__ __align__(16) uint64_t stage[INIT_WARPS * STAGE_ROWS * ROW];
+  __shared__ unsigned long long cta_ctr[CTA_INIT_CAND + 1];
+  const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
+  const uint32_t wbuf = smem_addr(stage) + warp * (STAGE_ROWS * ROW * 8);
+  const uint32_t cta = smem_addr(cta_ctr);
+  for (unsigned i = threadIdx.x; i < (unsigned)(CTA_INIT_CAND + 1); i += INIT_BLOCK) cta_ctr[i] = 0;
+  __syncthreads();
+  unsigned staged = 0;                     // rows in this warp's stage (warp-uniform)
+  unsigned long long sols = 0, cands = 0;
+  unsigned layout = 0;
+  int failed = 0;
+  const uint64_t stride = (uint64_t)gridDim.x * INIT_BLOCK;
+  // the loop bound is warp-uniform, so that the ballot and the stage insert see all 32 lanes
+  for (uint64_t base = (uint64_t)blockIdx.x * INIT_BLOCK + warp * 32; base < count; base += stride) {
+    const uint64_t i = base + lane;
+    const bool valid = i < count;
+    State s;
+    unsigned fail = 0;
+    const bool ok = valid && M::init_candidate(branch, first + i, s, fail);
+    if (fail) layout = fail;
+    const unsigned m = __ballot_sync(0xffffffffu, ok);
+    if (ok) {
+      const uint32_t row = wbuf + (staged + __popc(m & ((1u << lane) - 1))) * (ROW * 8);
+#pragma unroll
+      for (int k = 0; k < W; ++k) sts64(row + k * 8, s.w[k]);
+      sts64(row + W * 8, NO_PARENT);
+    }
+    staged += __popc(m);
+    sols += __popc(m);
+    cands += count - base < 32 ? count - base : 32;
+    if (staged >= (unsigned)STAGE_FLUSH) {
+      __syncwarp();
+      const int f = insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
+                                 p.viol_ring, wbuf, staged, cta);
+      if (f) failed = f;
+      staged = 0;
+      __syncwarp();
+    }
+  }
+  if (staged) {
+    __syncwarp();
+    const int f = insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
+                               p.viol_ring, wbuf, staged, cta);
+    if (f) failed = f;
+  }
+  layout = __reduce_or_sync(0xffffffffu, layout);
+  failed = __reduce_max_sync(0xffffffffu, failed);
+  if (lane == 0) {
+    if (sols) reds_add64(cta + CTA_INIT_GEN * 8, sols);
+    if (cands) reds_add64(cta + CTA_INIT_CAND * 8, cands);
+    // a solution that does not fit the layout is reported like a successor that does not: KMC_E_LAYOUT_OVERFLOW
+    if (layout) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)KMC_FAIL_LAYOUT);
+    else if (failed) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)failed);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned long long probes = cta_ctr[CTA_PROBES], oom = cta_ctr[CTA_OOM];
+    const unsigned long long g = cta_ctr[CTA_INIT_GEN], c = cta_ctr[CTA_INIT_CAND];
+    if (probes) atomicAdd(&p.ctr->probes, probes);
+    if (oom) atomicAdd(&p.ctr->out_of_model, oom);
+    if (g) {
+      atomicAdd(&p.ctr->generated, g);
+      atomicAdd(&p.ctr->init_generated, g);
+    }
+    if (c) atomicAdd(&p.ctr->init_candidates, c);
+  }
+}
+#endif
+
 __device__ __forceinline__ void st_release_sys(uint64_t* p, uint64_t v) {
   asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
@@ -1439,7 +1524,7 @@ __global__ void __launch_bounds__(SET_TILE) k_set_scatter(Params p, uint64_t fir
 // host side
 // ----------------------------------------------------------------------------------------
 struct LaunchRec {
-  int kind;  // 0 expand, 1 insert, 2 other, 3 set_spill's flushes and filters
+  int kind;  // 0 expand, 1 insert, 2 other, 3 set_spill's flushes and filters, 4 device Init (k_init)
   cudaEvent_t a, b;
 };
 
@@ -1901,14 +1986,15 @@ static int set_filter(Engine& E) {
 // flush).  The chunk then gets at most room / MAX_FANOUT states -- MAX_FANOUT is a true bound on a state's successors,
 // unlike fanout_bound, an assumed average -- so its successors, and so its inserts, fit the room whatever the states;
 // Params::region_rows (the KMC_E_CAND_FULL check of the expand kernel) is capped to the room as well.  After a failure
-// the chunk is left as it is: the run ends at the level end with that error.
-static int set_room(Engine& E, uint64_t* count, uint64_t* bound) {
+// the chunk is left as it is: the run ends at the level end with that error.  `per_item`: inserts one item of the chunk
+// can make (a state's successors; 1 for a candidate of the device Init).
+static int set_room(Engine& E, uint64_t* count, uint64_t* bound, uint64_t per_item = (uint64_t)M::MAX_FANOUT) {
   uint64_t tail, fail;
   int rc = read_tail(E, &tail, &fail);
   if (rc || fail) return rc;
   E.set_keys += tail - E.set_tail;
   E.set_tail = tail;
-  const uint64_t limit = set_limit(E), F = (uint64_t)M::MAX_FANOUT;
+  const uint64_t limit = set_limit(E), F = per_item;
   auto room = [&] { return E.set_keys < limit ? limit - E.set_keys : 0; };
   if (room() / F < std::min<uint64_t>(*count, std::max<uint64_t>(1, limit / F / 4))) {
     if ((rc = set_filter(E)) || (rc = set_flush(E))) return rc;
@@ -1976,6 +2062,12 @@ static void publish(Engine& E, const DevCounters& h, bool clamp) {
   st.set_host_keys = E.set_host_keys;
   st.set_filtered = E.set_filtered;
   st.set_link_bytes = E.set_link_bytes;
+#ifdef KMC_HAS_DEVICE_INIT
+  st.init_generated = h.init_generated;
+#else
+  st.init_generated = E.rank == 0 ? M::NUM_INIT : 0;
+#endif
+  st.init_candidates = h.init_candidates;
   E.site_generated.assign(h.site_generated, h.site_generated + M::NUM_SITES);
   E.action_distinct.assign(h.action_distinct, h.action_distinct + M::NUM_ACTIONS);
   E.inv_count.assign(h.inv_count, h.inv_count + 64);
@@ -2026,6 +2118,33 @@ static int seed_init(Engine& E) {
   CK(cudaStreamSynchronize(E.stream));
   return KMC_OK;
 }
+
+#ifdef KMC_HAS_DEVICE_INIT
+// Level 1 from the device form of Init: each branch's candidate space in chunks of at most region_rows candidates.  A
+// candidate yields at most one initial state, so a chunk's inserts are bounded like a frontier chunk's successors:
+// by the store (KMC_E_STORE_FULL) and, under set_spill, by the room left before the next flush, which may then fall
+// in the middle of level 1.
+static int seed_device_init(Engine& E) {
+  const Params p = E.params();
+  for (int b = 0; b < M::INIT_BRANCHES; ++b) {
+    for (uint64_t off = 0, cnt; off < M::INIT_SPACE[b]; off += cnt) {
+      cnt = std::min<uint64_t>(std::max<uint64_t>(1, E.region_rows), M::INIT_SPACE[b] - off);
+      uint64_t tail, fail, bound = 0;
+      int rc = read_tail(E, &tail, &fail);
+      if (rc) return rc;
+      if (fail) return KMC_OK;                     // the level end reports it
+      if (E.set_spill && (rc = set_room(E, &cnt, &bound, 1))) return rc;
+      if (cnt == 0) return KMC_OK;                 // (set_room failed: the level end reports it)
+      {
+        TimedLaunch t(E, 4);
+        k_init<<<grid_for(E, cnt, INIT_BLOCK, 8), INIT_BLOCK, 0, E.stream>>>(p, b, off, cnt);
+      }
+      CK(cudaGetLastError());
+    }
+  }
+  return KMC_OK;
+}
+#endif
 
 static int launch_insert(Engine& E, const uint64_t* rows, const unsigned long long* n_dev, uint64_t n_fixed,
                          uint64_t n_bound) {
@@ -2162,6 +2281,9 @@ static int write_checkpoint(Engine& E, const DevCounters& h) {
   // (before widths: a reader stops at widths.  Distinct per action is not written: it is the histogram of the
   // parent words, which recover reads anyway)
   for (int i = 0; i < M::NUM_SITES; ++i) fprintf(f, " %llu", (unsigned long long)h.site_generated[i]);
+#ifdef KMC_HAS_DEVICE_INIT
+  fprintf(f, "\ninit_generated %llu\ninit_candidates %llu", h.init_generated, h.init_candidates);
+#endif
   fprintf(f, "\nwidths");
   for (uint64_t w : E.widths) fprintf(f, " %llu", (unsigned long long)w);
   fprintf(f, "\n");
@@ -2209,6 +2331,8 @@ static int read_checkpoint(Engine& E, DevCounters* h) {
     else if (!strcmp(key, "deadlocks")) h->deadlocks = v;
     else if (!strcmp(key, "out_of_model")) h->out_of_model = v;
     else if (!strcmp(key, "probes")) h->probes = v;
+    else if (!strcmp(key, "init_generated")) h->init_generated = v;
+    else if (!strcmp(key, "init_candidates")) h->init_candidates = v;
   }
   fclose(f);
   if (digest != KMC_MODEL_DIGEST || words != (unsigned long long)W) {
@@ -2377,7 +2501,7 @@ static int collect_invariants(Engine& E, const DevCounters& h, uint64_t level, u
 }
 
 static void accumulate_timing(Engine& E, kmc_stats_t& st) {
-  st.gpu_ms_expand = st.gpu_ms_insert = st.gpu_ms_invariant = st.gpu_ms_set_spill = 0;
+  st.gpu_ms_expand = st.gpu_ms_insert = st.gpu_ms_invariant = st.gpu_ms_set_spill = st.gpu_ms_init = 0;
   st.launches_expand = st.launches_insert = st.launches_other = 0;
   for (const LaunchRec& r : E.launches) {
     float ms = 0;
@@ -2385,6 +2509,7 @@ static void accumulate_timing(Engine& E, kmc_stats_t& st) {
     if (r.kind == 0) { st.gpu_ms_expand += ms; st.launches_expand++; }
     else if (r.kind == 1) { st.gpu_ms_insert += ms; st.launches_insert++; }
     else if (r.kind == 3) st.gpu_ms_set_spill += ms;
+    else if (r.kind == 4) st.gpu_ms_init += ms;
     else { st.gpu_ms_invariant += ms; st.launches_other++; }
   }
 }
@@ -2431,9 +2556,15 @@ static int engine_run(Engine& E) {
     if ((rc = read_checkpoint(E, &h))) return rc;
     if ((rc = inv_begin(E, false))) return rc;
   } else {
+#ifdef KMC_HAS_DEVICE_INIT
+    if ((rc = seed_device_init(E))) return rc;
+    if (E.set_spill && (rc = set_filter(E))) return rc;         // before k_invariants sees the level
+    if ((rc = end_level(E, M::INIT_CANDIDATES, false, h))) return rc;
+#else
     if ((rc = seed_init(E))) return rc;
     if ((rc = launch_insert(E, E.cand, &E.ctr->cand_count[0], 0, M::NUM_INIT))) return rc;
     if ((rc = end_level(E, M::NUM_INIT, false, h))) return rc;
+#endif
     err = fail_to_error(h.fail);
     if (!err && h.viol_count && !E.cont) stopped = true;
   }
@@ -2495,6 +2626,21 @@ static int engine_run(Engine& E) {
 static int multi_create(kmcm_ctx* c, const char* options_json, int gpus);
 static int multi_run(kmcm_ctx* c);
 
+// A model whose Init is enumerated on the GPU (k_init) seeds level 1 on one GPU only: the sharded building blocks and
+// the "gpus" / world > 1 contexts refuse it with this text.
+static constexpr const char* DEVICE_INIT_ONE_GPU =
+    "this model's Init is enumerated on the GPU (device Init), which runs on one GPU: no \"gpus\" > 1, no world > 1, "
+    "no kmc_shard_* calls";
+static bool shard_refused(Engine& e) {
+#ifdef KMC_HAS_DEVICE_INIT
+  e.last_error = DEVICE_INIT_ONE_GPU;
+  return true;
+#else
+  (void)e;
+  return false;
+#endif
+}
+
 #define E (c->e)
 extern "C" {
 
@@ -2530,6 +2676,13 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
     return KMC_E_BADARG;
   }
   const bool gpus = json_num(options_json, "gpus", &d) && d > 1;
+#ifdef KMC_HAS_DEVICE_INIT
+  if (gpus || E.world > 1) {
+    E.last_error = DEVICE_INIT_ONE_GPU;
+    *out = c;
+    return KMC_E_BADARG;
+  }
+#endif
   if (E.set_spill && (gpus || E.world > 1)) {
     // each rank's set would need the keys of the others' host memory too
     E.last_error = "set_spill runs on one GPU (no \"gpus\" > 1, no world > 1)";
@@ -2588,6 +2741,9 @@ int kmcm_model_info(const kmcm_ctx*, kmc_model_info_t* out) {
   out->num_actions = M::NUM_ACTIONS;
   out->num_invariants = M::NUM_INVARIANTS;
   out->num_init = M::NUM_INIT;
+#ifdef KMC_HAS_DEVICE_INIT
+  out->init_candidates = M::INIT_CANDIDATES;
+#endif
   out->max_fanout = M::MAX_FANOUT;
   out->check_deadlock = M::CHECK_DEADLOCK;
   out->exact = EXACT_SET ? 1 : 0;
@@ -2802,7 +2958,7 @@ int kmcm_fpset_size(const kmcm_ctx* c_, uint64_t* out) {
 // None of them runs on a set_spill context: they insert without the filter that keeps the store free of states whose
 // keys are in host memory.
 int kmcm_shard_begin(kmcm_ctx* c) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   int rc = engine_reset(E);
   if (rc) return rc;
@@ -2813,7 +2969,7 @@ int kmcm_shard_begin(kmcm_ctx* c) {
 }
 
 int kmcm_shard_buffers(kmcm_ctx* c, kmc_shard_buffers_t* out) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !out) return KMC_E_BADARG;
   out->cand = E.cand;
   out->region_rows = E.region_rows;
@@ -2825,13 +2981,13 @@ int kmcm_shard_buffers(kmcm_ctx* c, kmc_shard_buffers_t* out) {
 }
 
 int kmcm_shard_seed_init(kmcm_ctx* c) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   return seed_init(E);
 }
 
 int kmcm_shard_expand(kmcm_ctx* c, uint64_t first, uint64_t count) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   if (count > E.chunk_states) {
     E.last_error = "expand chunk larger than chunk_states";
@@ -2842,7 +2998,7 @@ int kmcm_shard_expand(kmcm_ctx* c, uint64_t first, uint64_t count) {
 }
 
 int kmcm_shard_counts(kmcm_ctx* c, uint64_t* host_counts) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !host_counts) return KMC_E_BADARG;
   unsigned long long tmp[MAX_WORLD];
   CK(cudaMemcpyAsync(tmp, E.ctr->cand_count, sizeof(tmp), cudaMemcpyDeviceToHost, E.stream));
@@ -2852,13 +3008,13 @@ int kmcm_shard_counts(kmcm_ctx* c, uint64_t* host_counts) {
 }
 
 int kmcm_shard_reset_cand(kmcm_ctx* c) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   return reset_cand(E);
 }
 
 int kmcm_shard_insert(kmcm_ctx* c, const uint64_t* rows_dev, uint64_t rows, uint64_t* new_tail) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   if (rows) {
     int rc = launch_insert(E, rows_dev, nullptr, rows, rows);
@@ -2875,7 +3031,7 @@ int kmcm_shard_insert(kmcm_ctx* c, const uint64_t* rows_dev, uint64_t rows, uint
 }
 
 int kmcm_shard_level_done(kmcm_ctx* c, uint64_t* level_first, uint64_t* level_count) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   DevCounters h;
   int rc = end_level(E, std::max<uint64_t>(E.level_count * 2, 1024), true, h);
@@ -2887,7 +3043,7 @@ int kmcm_shard_level_done(kmcm_ctx* c, uint64_t* level_first, uint64_t* level_co
 
 // ---- fused exchange over peer memory ---------------------------------------------------------
 int kmcm_shard_ipc_handle(kmcm_ctx* c, void* out64) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !out64 || !E.inbox) return KMC_E_BADARG;
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   cudaIpcMemHandle_t h;
@@ -2898,7 +3054,7 @@ int kmcm_shard_ipc_handle(kmcm_ctx* c, void* out64) {
 }
 
 int kmcm_shard_open_peers(kmcm_ctx* c, const void* handles, uint32_t world) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !handles || world != E.world || !E.inbox) return KMC_E_BADARG;
   CK(cudaSetDevice(E.device));
   for (uint32_t r = 0; r < world; ++r) {
@@ -2919,7 +3075,7 @@ int kmcm_shard_open_peers(kmcm_ctx* c, const void* handles, uint32_t world) {
 // expand a frontier chunk, storing every successor row directly into its owner's inbox, then
 // publish the per-owner row counts into the owners' inbox headers (both on the engine stream)
 int kmcm_shard_expand_p2p(kmcm_ctx* c, uint64_t first, uint64_t count) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   if (count > E.chunk_states) return KMC_E_BADARG;
   int rc = reset_cand(E);
@@ -2937,7 +3093,7 @@ int kmcm_shard_expand_p2p(kmcm_ctx* c, uint64_t first, uint64_t count) {
 
 // seed: the initial states go through the same inbox path (rank 0 contributes them)
 static int seed_p2p(kmcm_ctx* c, bool publish) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   CK(cudaSetDevice(E.device));
   unsigned long long counts[MAX_WORLD] = {0};
@@ -2973,7 +3129,7 @@ int kmcm_shard_seed_p2p(kmcm_ctx* c) { return seed_p2p(c, true); }
 // insert everything the peers stored into the current inbox buffer, then switch buffers.
 // The caller must have put a cross-rank barrier on the stream between expand_p2p and this call.
 int kmcm_shard_insert_p2p(kmcm_ctx* c) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   Params p = E.params();
   {
@@ -2991,7 +3147,7 @@ int kmcm_shard_insert_p2p(kmcm_ctx* c) {
 //   wait until every source is ready for this round; insert from the own inbox; publish done
 // Every rank must call it the same number of times (count = 0 on ranks without work).
 int kmcm_shard_round_p2p(kmcm_ctx* c, uint64_t first, uint64_t count, int seed) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !E.peers_open) return KMC_E_STATE;
   if (count > E.chunk_states) return KMC_E_BADARG;
   CK(cudaSetDevice(E.device));
@@ -3022,7 +3178,7 @@ int kmcm_shard_round_p2p(kmcm_ctx* c, uint64_t first, uint64_t count, int seed) 
 // for all summaries, copy the board to pinned host memory, ONE stream synchronisation.  board_out receives
 // world x 8 words: {level id, new states, violations, store tail, generated, fail, deadlocks, -} per rank.
 int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !E.peers_open || !board_out) return KMC_E_STATE;
   CK(cudaSetDevice(E.device));
   int rc = launch_invariants(E, E.level_first + E.level_count, std::max<uint64_t>(E.level_count * 2, 1024));
@@ -3070,13 +3226,13 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
 // same-process peers (one context per GPU in one process): direct pointers instead of CUDA IPC handles.
 // inboxes[r] = the value kmcm_shard_inbox_ptr returned for rank r's context.
 int kmcm_shard_inbox_ptr(kmcm_ctx* c, void** out) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !out || !E.inbox_alloc) return KMC_E_BADARG;
   *out = E.inbox_alloc;
   return KMC_OK;
 }
 int kmcm_shard_open_peers_direct(kmcm_ctx* c, void* const* inboxes, const int* devices, uint32_t world) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c || !inboxes || !devices || world != E.world || !E.inbox_alloc) return KMC_E_BADARG;
   CK(cudaSetDevice(E.device));
   for (uint32_t r = 0; r < world; ++r) {
@@ -3096,7 +3252,7 @@ int kmcm_shard_open_peers_direct(kmcm_ctx* c, void* const* inboxes, const int* d
 }
 
 int kmcm_shard_sync(kmcm_ctx* c) {
-  if (c && E.set_spill) return KMC_E_BADARG;
+  if (c && (E.set_spill || shard_refused(E))) return KMC_E_BADARG;
   if (!c) return KMC_E_BADARG;
   CK(cudaEventRecord(E.ev_end, E.stream));
   DevCounters h;

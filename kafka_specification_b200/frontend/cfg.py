@@ -27,6 +27,8 @@ valid TLC configuration:
     \\* kspec: PREFIX replicaLog records endOffset
                                                   in every record of the variable, `records[o]` is the Nil alternative
                                                   exactly for o >= `endOffset` (checked), so Nil needs no code of its own
+    \\* kspec: INIT DEVICE                         enumerate Init on the GPU (lower/init_device.py) even when it has
+                                                  fewer candidates than the threshold that selects that form by itself
 """
 from __future__ import annotations
 
@@ -68,6 +70,7 @@ class Config:
     type_hints: dict[str, tuple] = field(default_factory=dict)       # var -> ("\\in" | "\\subseteq", TLA+ expression text)
     keyed: dict[str, str] = field(default_factory=dict)              # var -> key field
     prefix: dict[str, tuple] = field(default_factory=dict)           # var -> (array field, length field)
+    init_device: bool = False                                        # kspec pragma INIT DEVICE: Init is enumerated on the GPU
     source: str = ""
 
 
@@ -199,6 +202,9 @@ def parse_cfg(text: str) -> Config:
         m = re.match(r"KEYED\s+(\w+)\s+BY\s+(\w+)\s*$", p)
         if m:
             cfg.keyed[m.group(1)] = m.group(2)
+            continue
+        if re.match(r"INIT\s+DEVICE\s*$", p):
+            cfg.init_device = True
             continue
         m = re.match(r"PREFIX\s+(\w+)\s+(\w+)\s+(\w+)\s*$", p)
         if m:

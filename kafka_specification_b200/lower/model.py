@@ -19,6 +19,7 @@ from ..frontend.tla_parser import parse_expression_text
 from ..frontend.values import FnVal, fmt, sort_key
 from . import layout as L
 from .compiler import Block, Closure, Lowerer, Marker, Thunk, render
+from .init_device import device_init
 from .svals import LowerError, SLazy, is_atom_const, is_const, is_int_const
 
 LOWERING_VERSION = 3
@@ -362,6 +363,7 @@ def _init_states(lw: Lowerer, init_expr) -> list[dict]:
     out: list[dict] = []
 
     def rec(items, st):
+        lw.cur = st                 # what an operator argument or a LET definition reads when it is forced
         if not items:
             for v in lw.variables:
                 if v not in st:
@@ -413,6 +415,7 @@ def _init_states(lw: Lowerer, init_expr) -> list[dict]:
             raise LowerError("Init contains a non-constant condition")
 
     rec([(init_expr, lw.root, None, {})], {})
+    lw.cur = None
     return out
 
 
@@ -558,13 +561,20 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     lw.layout = lay
 
     init_e, next_e = _resolve_init_next(lw)
-    inits = _init_states(lw, init_e)
-    if not inits:
-        raise LowerError("Init has no solution")
-    init_words = [lay.py_pack(st) for st in inits]
-    for st, wds in zip(inits, init_words):
-        if lay.py_unpack(wds) != st:
-            raise LowerError("layout round-trip of an initial state failed")
+    dev = device_init(lw, init_e, cfg)
+    init_lines: list[str] = []
+    if dev is not None:
+        # device form: k_init decodes, filters and packs the candidates; the header has no table
+        init_words = []
+        init_lines = dev.emit()
+    else:
+        inits = _init_states(lw, init_e)
+        if not inits:
+            raise LowerError("Init has no solution")
+        init_words = [lay.py_pack(st) for st in inits]
+        for st, wds in zip(inits, init_words):
+            if lay.py_unpack(wds) != st:
+                raise LowerError("layout round-trip of an initial state failed")
 
     # expand()
     lw.begin_function()
@@ -679,7 +689,8 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
     name = name or module
     if len(lw.actions) > 255:
         raise LowerError(f"{len(lw.actions)} sub-actions: the parent word holds the action id in 8 bits (<= 255)")
-    body_digest = hashlib.sha256(("\n".join(expand_lines + inv_lines + con_lines + sym_lines) + cfg_text).encode()).hexdigest()[:16]
+    # (the device form's code is part of what a checkpoint is checked against; a table model hashes what it always did)
+    body_digest = hashlib.sha256(("\n".join(expand_lines + inv_lines + con_lines + sym_lines + init_lines) + cfg_text).encode()).hexdigest()[:16]
     unpack = lw.unpack_lines()
 
     parts = [HEADER_PROLOGUE.format(
@@ -688,10 +699,13 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
         num_actions=max(1, len(lw.actions)), num_invariants=len(cfg.invariants),
         num_constraints=len(cfg.constraints), num_init=len(init_words), max_fanout=max(1, max_fanout),
         check_deadlock="true" if cfg.check_deadlock else "false")]
-    parts.append("static const uint64_t INIT_STATES[NUM_INIT][W] = {")
-    for wds in init_words:
-        parts.append("  {" + ", ".join(f"0x{w:x}ull" for w in wds) + "},")
-    parts.append("};")
+    if dev is not None:
+        parts.extend(init_lines)
+    else:
+        parts.append("static const uint64_t INIT_STATES[NUM_INIT][W] = {")
+        for wds in init_words:
+            parts.append("  {" + ", ".join(f"0x{w:x}ull" for w in wds) + "},")
+        parts.append("};")
     parts.append("/* successor enumeration: sink.emit(const State&, int action) per successor; sink.fail(code) on a layout trap.")
     parts.append("   Two equivalent forms (tests prove they enumerate the same multiset):")
     parts.append("   one-phase   expand() = expand_group<0..NUM_GROUPS-1> in order; a group is a slice of the Next disjuncts /")
@@ -801,5 +815,6 @@ def lower_model(module: str, search_dirs: list[str], cfg_text: str, name: str | 
         invariants=list(cfg.invariants), constraints=list(cfg.constraints),
         check_deadlock=cfg.check_deadlock, max_fanout=max(1, max_fanout), warnings=lw.warnings,
         digest=body_digest, lowerer=lw, variables=list(lw.variables),
-        sites=[{"action": a} for a in site_action], init=_init_info(lw, init_e, module),
+        sites=[{"action": a} for a in site_action],
+        init={**_init_info(lw, init_e, module), **(dev.describe() if dev is not None else {})},
         invariants_header=invariants_header)

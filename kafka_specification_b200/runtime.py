@@ -43,6 +43,7 @@ class Stats(ctypes.Structure):
         ("complete", ctypes.c_uint64), ("gpu_ms_invariant", ctypes.c_double), ("slot_bytes", ctypes.c_uint64),
         ("set_flushes", ctypes.c_uint64), ("set_host_keys", ctypes.c_uint64), ("set_filtered", ctypes.c_uint64),
         ("gpu_ms_set_spill", ctypes.c_double), ("set_link_bytes", ctypes.c_uint64),
+        ("init_generated", ctypes.c_uint64), ("init_candidates", ctypes.c_uint64), ("gpu_ms_init", ctypes.c_double),
     ]
 
     def as_dict(self) -> dict:
@@ -63,7 +64,7 @@ class ModelInfo(ctypes.Structure):
     _fields_ = [("words", ctypes.c_int32), ("state_bits", ctypes.c_int32), ("num_actions", ctypes.c_int32),
                 ("num_invariants", ctypes.c_int32), ("num_init", ctypes.c_int32), ("max_fanout", ctypes.c_int32),
                 ("check_deadlock", ctypes.c_int32), ("exact", ctypes.c_int32),
-                ("name", ctypes.c_char * 128), ("digest", ctypes.c_char * 32)]
+                ("name", ctypes.c_char * 128), ("digest", ctypes.c_char * 32), ("init_candidates", ctypes.c_uint64)]
 
 
 class ShardBuffers(ctypes.Structure):
@@ -195,6 +196,9 @@ class RunResult:
     trace: list[dict] = field(default_factory=list)
     # with "continue": every violated invariant (Checker.invariant_reports), ordered by (level, cfg index)
     invariant_violations: list[dict] = field(default_factory=list)
+    # Init solutions, duplicates included, and (device Init) the candidate assignments decoded on the GPU
+    init_generated: int = 0
+    init_candidates: int = 0
 
 
 class Checker:
@@ -292,8 +296,13 @@ class Checker:
         actions = [{"name": a["name"], "module": a.get("module"), "location": {k: a[k] for k in ("line", "col", "end_line", "end_col") if k in a},
                     "generated": int(gen[i]), "distinct": int(dist[i])} for i, a in enumerate(acts)]
         init_distinct = st["distinct"] - sum(a["distinct"] for a in actions)
-        return {"init": {**self.meta.get("init", {"name": "Init"}), "distinct": init_distinct,
-                         "generated": len(self.meta["init_states"])},
+        init = dict(self.meta.get("init", {"name": "Init"}))
+        # a device-form Init (model.json init.device) has no table: its generated count comes from the run
+        device = bool(init.pop("device", False))
+        init.pop("candidates", None)
+        init.pop("branches", None)
+        return {"init": {**init, "distinct": init_distinct,
+                         "generated": st["init_generated"] if device else len(self.meta["init_states"])},
                 "actions": actions, "sites": [int(site[i]) for i in range(n_s.value)], "complete": bool(complete.value)}
 
     def violation(self) -> dict | None:
@@ -361,7 +370,8 @@ class Checker:
         reports = self.invariant_reports() if self.cont and len(self.meta["invariants"]) <= 64 else []
         return RunResult(distinct=st["distinct"], generated=st["generated"], depth=st["depth"], queue=st["queue"],
                          deadlocks=st["deadlocks"], complete=bool(st["complete"]), levels=self.level_widths(),
-                         stats=st, violation=viol, trace=self.trace() if viol else [], invariant_violations=reports)
+                         stats=st, violation=viol, trace=self.trace() if viol else [], invariant_violations=reports,
+                         init_generated=st["init_generated"], init_candidates=st["init_candidates"])
 
     def violation_record(self):
         """(packed words, parent word) of this rank's offending state, or None."""

@@ -240,6 +240,10 @@ def main(argv=None) -> int:
         msg("general", f"Error: {e}", 1)
         return 1
     n_init = len(model.init_states)
+    if model.init.get("device"):
+        # the device form of Init has no table: the initial states are level 1 of the run (all of the states found
+        # when the run stopped in level 1)
+        n_init = r.levels[0] if r.levels else r.distinct
     msg("init_done", f"Finished computing initial states: {n_init} distinct state{'s' if n_init != 1 else ''} generated.")
     blocks, exit_code = error_messages(r.violation, r.trace, r.invariant_violations)
     for kind, text, cls in blocks:
