@@ -110,16 +110,18 @@ def compare_runs(fused, ref, symmetric=False):
             assert np.array_equal(x, y), f"level {depth}"
 
 
-def audited_run(name, details=False, **opts):
+def audited_run(name, details=False, init_rows=None, **opts):
     """One kmc_run and the audit of its whole store (store_audit.audit_checker): (RunResult, audit report).  The report
     holds the run's violation record ("record"); with `details` also its coverage and the TLC text of every stored
-    state ("coverage", "texts").  A "check_deadlock" option goes to the audit as well."""
+    state ("coverage", "texts").  A "check_deadlock" option goes to the audit as well; `init_rows` are the generated
+    initial states of a device Init too large for the audit to enumerate."""
     from store_audit import audit_checker
     with checker(name, **opts) as ck:
         r = ck.run()
-        # the initial states only (none when recovering): the successors are inserted by the expand kernel
-        assert r.stats["launches_insert"] == (0 if "recover" in opts else 1)
-        rep = audit_checker(ck, r.levels, r.distinct, check_deadlock=opts.get("check_deadlock"))
+        # the initial states only (none when recovering, none from k_init): the successors are inserted by the expand
+        # kernel
+        assert r.stats["launches_insert"] == (0 if "recover" in opts or ck.info.init_candidates else 1)
+        rep = audit_checker(ck, r.levels, r.distinct, check_deadlock=opts.get("check_deadlock"), init_rows=init_rows)
         if details:
             rep["coverage"] = ck.coverage()
             rep["texts"] = [ck.decoder.text(row) for row in ck.copy_states(0, r.distinct)]

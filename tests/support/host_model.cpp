@@ -4,7 +4,7 @@
 //   g++ -O2 -std=c++17 -shared -fPIC -DKMC_MODEL_HEADER='"model.h"' -DKMC_INVARIANTS_HEADER='"invariants.h"' host_model.cpp
 // It holds
 //   hm_*     the model's facts and per-state calls: successors under either form of Next, invariants (first violated and
-//            the mask of all violated), constraints, initial states, canonical forms
+//            the mask of all violated), constraints, initial states (either form of Init), canonical forms
 //   hm_bfs   a level-ordered sequential BFS that stores its states as the engine does, with the run's statistics
 //   audit_*  the whole-store audit of a finished or stopped GPU run
 //   hs_*     a stand-in for one rank of the sharded engine (kafka_specification_b200/sharded.py's CPU tests)
@@ -145,6 +145,68 @@ void hm_canonicalize(const uint64_t* states, uint64_t n, uint64_t* out) {
 }
 }  // extern "C"
 
+// ================================================================================================ Init
+// Both forms of Init as one list of generated initial states (duplicates included, as TLC counts them): the host
+// form's INIT_STATES table, or every solution of every candidate of every branch of the device form, in branch and
+// candidate order -- the order k_init counts them in, though it inserts them in any order.
+namespace {
+#ifdef KMC_HAS_DEVICE_INIT
+constexpr int INIT_BRANCHES = M::INIT_BRANCHES;
+uint64_t init_space(int b) { return M::INIT_SPACE[b]; }
+#else
+constexpr int INIT_BRANCHES = 0;
+uint64_t init_space(int) { return 0; }
+#endif
+// 1: a solution, packed into s; 0: rejected by a filter; -code: a solution that traps the layout
+int init_candidate(int b, uint64_t idx, State& s) {
+#ifdef KMC_HAS_DEVICE_INIT
+  unsigned fail = 0;
+  memset(s.w, 0, sizeof(s.w));
+  const bool ok = M::init_candidate(b, idx, s, fail);
+  if (fail) return -(int)fail;
+  return ok ? 1 : 0;
+#else
+  (void)b, (void)idx, (void)s;
+  return 0;
+#endif
+}
+// Calls f(state) for every generated initial state; returns 0, or the code of the first layout trap (and stops there).
+template <class F>
+int for_each_init(F&& f) {
+  for (int i = 0; i < M::NUM_INIT; ++i) f(load(M::INIT_STATES[i]));
+  State s;
+  for (int b = 0; b < INIT_BRANCHES; ++b)
+    for (uint64_t i = 0; i < init_space(b); ++i) {
+      const int r = init_candidate(b, i, s);
+      if (r < 0) return -r;
+      if (r > 0) f(s);
+    }
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+int hm_init_branches() { return INIT_BRANCHES; }
+uint64_t hm_init_space(int b) { return b >= 0 && b < INIT_BRANCHES ? init_space(b) : 0; }
+// Candidate idx of branch b of the device form: 1 (a solution, its words in out), 0 (rejected) or -code (a solution
+// that does not fit the layout).
+int hm_init_candidate(int b, uint64_t idx, uint64_t* out) {
+  State s;
+  const int r = init_candidate(b, idx, s);
+  if (r > 0) memcpy(out, s.w, sizeof(s.w));
+  return r;
+}
+// Every generated initial state of either form: the first `cap` of them into out, their number into *n; returns 0 or
+// the code of a layout trap.
+int hm_init_solutions(uint64_t* out, uint64_t cap, uint64_t* n) {
+  *n = 0;
+  return for_each_init([&](const State& s) {
+    if (*n < cap) memcpy(out + *n * W, s.w, sizeof(s.w));
+    ++*n;
+  });
+}
+}  // extern "C"
+
 // ================================================================================================ the BFS
 namespace {
 enum { T_GENERATED, T_DEADLOCKS, T_FAIL, T_COMPLETE, T_EXPANDED, T_MAX_FANOUT, T_FIRST_INV, T_FIRST_LEVEL, T_MISMATCHES,
@@ -213,9 +275,15 @@ void hm_bfs(int sites, uint64_t stop_at) {
     B.parents.push_back(pw);
     check(s, level);
   };
-  for (int i = 0; i < M::NUM_INIT; ++i) {
+  // every solution of the device form is generated; one that does not fit the layout traps like a successor
+  const int init_fail = for_each_init([&](const State& s) {
     t[T_GENERATED]++;
-    reach(load(M::INIT_STATES[i]), NO_PARENT, 1);
+    reach(s, NO_PARENT, 1);
+  });
+  if (init_fail) {
+    t[T_FAIL] = (uint64_t)init_fail;
+    t[T_COMPLETE] = 0;
+    return;
   }
   Sink sink;
   for (uint64_t first = 0; first < B.parents.size();) {
@@ -259,7 +327,8 @@ void hm_bfs_clear() { g_bfs = Bfs(); }
 // ================================================================================================ the store audit
 // The audit checks, state by state, what the engine's bookkeeping claims about a store (the stored states and parent
 // words of one rank, or the union of several ranks' stores, each state's BFS level and the number of expanded levels):
-//   init        level 1 = the in-model INIT_STATES, one per identity, parent word NO_PARENT
+//   init        level 1 = the in-model initial states (INIT_STATES, or the device form's solutions), one per identity,
+//               parent word NO_PARENT
 //   edges       a state of level L >= 2 names a parent of level L-1 (rank, index), an action id < NUM_ACTIONS, and its
 //               exact words are a successor of that parent labelled with that action, under expand() AND the two-phase
 //               form
@@ -335,17 +404,22 @@ struct ViolationSink {
 std::vector<uint64_t> g_viol_rows;
 }  // namespace
 
+// Above this many candidates the audit does not enumerate the device form of Init: the caller passes the initial states.
+constexpr uint64_t AUDIT_MAX_INIT_CANDIDATES = 1ull << 32;
+
 extern "C" {
 // Returns 0 when every check passes, else 1 with "<check>: <what>" in msg.  level[i] is state i's BFS level (1 = Init);
-// levels 1..n_expanded were expanded.  Outputs (also on failure, as far as computed):
-//   totals[0] generated (NUM_INIT + successors of the expanded states)   totals[1] deadlocks of the expanded states
+// levels 1..n_expanded were expanded.  The generated initial states (duplicates included) are init_rows[n_init_rows]
+// when init_rows is given, else the model's own (INIT_STATES, or every candidate of the device form up to
+// AUDIT_MAX_INIT_CANDIDATES).  Outputs (also on failure, as far as computed):
+//   totals[0] generated (initial states + successors of the expanded states)   totals[1] deadlocks of the expanded states
 //   totals[2] out-of-model (initial states and successors)
 //   act_gen[NUM_ACTIONS], site_gen[NUM_SITES]: successors per action / per emit site
 //   viol_counts[n_expanded + 1]: violators recorded at each level end; audit_violator_rows then returns those of the
 //   first level end that has any
 int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t* level, uint64_t n, const uint64_t* rank_off,
-                uint32_t n_ranks, uint32_t n_expanded, int check_deadlock, uint64_t* totals,
-                uint64_t* act_gen, uint64_t* site_gen, uint64_t* viol_counts, char* msg, size_t msg_cap) {
+                uint32_t n_ranks, uint32_t n_expanded, int check_deadlock, const uint64_t* init_rows, uint64_t n_init_rows,
+                uint64_t* totals, uint64_t* act_gen, uint64_t* site_gen, uint64_t* viol_counts, char* msg, size_t msg_cap) {
   const Store S{states, parents, level, n, rank_off, n_ranks};
   memset(totals, 0, 3 * sizeof(uint64_t));
   memset(act_gen, 0, sizeof(uint64_t) * M::NUM_ACTIONS);
@@ -359,19 +433,34 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
       return report(msg, msg_cap, "levels: the level bounds are not ordered");
 
   // ---- init: level 1 is the set of in-model initial states, one per identity
-  StateSet init_ids;
-  totals[0] = M::NUM_INIT;
-  for (int i = 0; i < M::NUM_INIT; ++i) {
-    const State s = load(M::INIT_STATES[i]);
+  StateSet init_ids, init_words;
+  auto add_init = [&](const State& s) {
+    totals[0]++;
     if (!kept(s)) {
       totals[2]++;
       if (M::NUM_INVARIANTS > 0) {
         const int inv = M::first_violated_invariant(s);
         if (inv >= 0) V.add(0, s, NO_PARENT, (uint64_t)inv);
       }
-      continue;
+      return;
     }
+    init_words.insert(s);
     init_ids.insert(canon(s));
+  };
+  if (init_rows) {
+    for (uint64_t i = 0; i < n_init_rows; ++i) add_init(load(init_rows + i * W));
+  } else {
+    uint64_t candidates = 0;
+    for (int br = 0; br < INIT_BRANCHES; ++br) candidates += init_space(br);
+    if (candidates > AUDIT_MAX_INIT_CANDIDATES) {
+      snprintf(b, sizeof(b), "init: the device form has %llu candidates, more than the audit enumerates: pass the initial states",
+               (unsigned long long)candidates);
+      return report(msg, msg_cap, b);
+    }
+    if (const int code = for_each_init(add_init)) {
+      snprintf(b, sizeof(b), "init: a solution of the device form traps the layout (code %d)", code);
+      return report(msg, msg_cap, b);
+    }
   }
   uint64_t n_level1 = 0;
   for (uint64_t i = 0; i < n; ++i) {
@@ -385,9 +474,7 @@ int audit_store(const uint64_t* states, const uint64_t* parents, const uint32_t*
     }
     ++n_level1;
     const State s = S.at(i);
-    bool is_init = false;
-    for (int k = 0; k < M::NUM_INIT && !is_init; ++k) is_init = memcmp(s.w, M::INIT_STATES[k], sizeof(s.w)) == 0;
-    if (!is_init || parents[i] != NO_PARENT || !init_ids.count(canon(s))) {
+    if (!init_words.count(s) || parents[i] != NO_PARENT || !init_ids.count(canon(s))) {
       snprintf(b, sizeof(b), "init: level-1 state %llu [%s] parent word %016llx is not an in-model initial state with NO_PARENT",
                (unsigned long long)i, words_text(s).c_str(), (unsigned long long)parents[i]);
       return report(msg, msg_cap, b);

@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
-from kafka_specification_b200.build import registry, tla_search_dirs  # noqa: E402
+from kafka_specification_b200.build import device_init_registry, registry, tla_search_dirs  # noqa: E402
 from kafka_specification_b200.lower.model import LoweredModel, lower_model  # noqa: E402,F401
 
 BUILD = os.path.join(ROOT, "build", "hosttest")
@@ -38,11 +38,15 @@ SIGNATURES = {
     "hm_mask": (_u64, [_vp]),
     "hm_in_model": (_i32, [_vp]),
     "hm_init_state": (None, [_i32, _vp]),
+    "hm_init_branches": (_i32, []),
+    "hm_init_space": (_u64, [_i32]),
+    "hm_init_candidate": (_i32, [_i32, _u64, _vp]),
+    "hm_init_solutions": (_i32, [_vp, _u64, _vp]),
     "hm_canonicalize": (None, [_vp, _u64, _vp]),
     "hm_bfs": (None, [_i32, _u64]),
     "hm_bfs_array": (_u64p, [_i32, _vp]),
     "hm_bfs_clear": (None, []),
-    "audit_store": (_i32, [_vp, _vp, _vp, _u64, _vp, _u32, _u32, _i32, _vp, _vp, _vp, _vp, ctypes.c_char_p,
+    "audit_store": (_i32, [_vp, _vp, _vp, _u64, _vp, _u32, _u32, _i32, _vp, _u64, _vp, _vp, _vp, _vp, ctypes.c_char_p,
                            ctypes.c_size_t]),
     "audit_violator_rows": (_u64, [_vp, _u64]),
     "hs_create": (_vp, [_u32, _u32]),
@@ -83,9 +87,9 @@ def _library_path(header_text: str, invariants_text: str) -> str:
 
 @functools.lru_cache(maxsize=None)
 def lower_registered(name: str) -> LoweredModel:
-    """The registered model `name` (build.registry()) lowered from its module and cfg as build() lowers it, once per
-    process; `lower_registered.__wrapped__(name)` lowers it afresh."""
-    spec = registry()[name]
+    """The registered model `name` (build.registry() or build.device_init_registry()) lowered from its module and cfg
+    as build() lowers it, once per process; `lower_registered.__wrapped__(name)` lowers it afresh."""
+    spec = {**registry(), **device_init_registry()}[name]
     with open(os.path.join(ROOT, spec["cfg"])) as f:
         return lower_model(spec["module"], tla_search_dirs(), f.read(), name=name)
 
@@ -116,6 +120,7 @@ class HostModel:
         self.check_deadlock = bool(lib.hm_check_deadlock())
         self.digest = lib.hm_digest().decode()
         self.site_action = [lib.hm_site_action(i) for i in range(self.num_sites)]
+        self.init_space = [int(lib.hm_init_space(b)) for b in range(lib.hm_init_branches())]   # device form only
 
     @classmethod
     def from_lowered(cls, model: LoweredModel):
@@ -171,6 +176,27 @@ class HostModel:
         for i in range(self.num_init):
             self.lib.hm_init_state(i, out[i].ctypes.data)
         return out
+
+    def init_candidate(self, branch: int, idx: int) -> tuple[str, np.ndarray | None]:
+        """Candidate idx of one branch of the device form of Init: ("solution", its words), ("rejected", None) or
+        ("trapped", None) for a solution that does not fit the layout."""
+        out = np.zeros(self.words, dtype=np.uint64)
+        r = self.lib.hm_init_candidate(branch, idx, out.ctypes.data)
+        return ("solution", out) if r > 0 else ("rejected", None) if r == 0 else ("trapped", None)
+
+    def init_solutions(self) -> np.ndarray:
+        """[n, W] every generated initial state of either form of Init, duplicates included: the table, or every
+        solution of every candidate of every branch in branch and candidate order."""
+        cap = 1 << 16
+        while True:
+            out = np.zeros((cap, self.words), dtype=np.uint64)
+            n = ctypes.c_uint64()
+            code = self.lib.hm_init_solutions(out.ctypes.data, cap, ctypes.byref(n))
+            if code:
+                raise RuntimeError(f"{self.name}: an initial state traps the layout (code {code})")
+            if n.value <= cap:
+                return out[: n.value]
+            cap = n.value
 
     def canonicalize(self, rows: np.ndarray) -> np.ndarray:
         rows = np.ascontiguousarray(rows, dtype=np.uint64).reshape(-1, self.words)

@@ -171,3 +171,16 @@ def run_bfs_by_action(module: str, search_dirs: list[str], cfg_text: str) -> dic
         tla_interp.Interp = saved
     res["per_action"] = dict(interps[0].generated)
     return res
+
+
+def init_states(module: str, cfg_text: str, dirs: list[str]) -> Counter:
+    """Oracle A's initial states of a spec, as the multiset of their TLC texts (/\\ v = value, one line per variable)."""
+    import tla_interp
+    from kafka_specification_b200.frontend.cfg import parse_cfg
+    from kafka_specification_b200.frontend.modules import load_root
+    from kafka_specification_b200.frontend.values import fmt
+    cfg = parse_cfg(cfg_text)
+    root = load_root(module, dirs)
+    it = tla_interp.Interp(root, cfg)
+    init_e, _ = tla_interp.resolve_init_next(root, cfg)
+    return Counter("\n".join(f"/\\ {v} = {fmt(st[v])}" for v in it.variables) for st in it.init_states(init_e))

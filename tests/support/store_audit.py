@@ -151,10 +151,12 @@ class AuditLib(HostModel):
         return {"states": r["states"], "parents": r["parents"], "widths": r["widths"], "n_expanded": r["n_expanded"]}
 
     def check_store(self, states, parents, widths, n_expanded: int, *, check_deadlock: bool,
-                    rank_widths: list[list[int]] | None = None) -> dict:
+                    rank_widths: list[list[int]] | None = None, init_rows: np.ndarray | None = None) -> dict:
         """Init, edges, uniqueness and closure of a store; returns the recomputed totals and the violators of the first
         level end that has any.  `widths` are the level widths of one rank's store; for the union of several ranks'
-        stores (concatenated in rank order) pass `rank_widths`, one list per rank."""
+        stores (concatenated in rank order) pass `rank_widths`, one list per rank.  `init_rows` are the generated
+        initial states (duplicates included) when the audit is not to enumerate them itself: a device form of Init
+        with more than 2^32 candidates, whose solutions the caller knows in closed form."""
         states = np.ascontiguousarray(states, dtype=np.uint64).reshape(-1, self.words)
         parents = np.ascontiguousarray(parents, dtype=np.uint64)
         per_rank = rank_widths if rank_widths is not None else [list(widths)]
@@ -172,8 +174,12 @@ class AuditLib(HostModel):
         site_gen = np.zeros(max(self.num_sites, 1), dtype=np.uint64)
         viol_counts = np.zeros(n_expanded + 1, dtype=np.uint64)
         msg = ctypes.create_string_buffer(1024)
+        if init_rows is not None:
+            init_rows = np.ascontiguousarray(init_rows, dtype=np.uint64).reshape(-1, self.words)
         rc = self.lib.audit_store(states.ctypes.data, parents.ctypes.data, level.ctypes.data, n, rank_off.ctypes.data,
-                                  len(per_rank), n_expanded, 1 if check_deadlock else 0, totals.ctypes.data,
+                                  len(per_rank), n_expanded, 1 if check_deadlock else 0,
+                                  None if init_rows is None else init_rows.ctypes.data,
+                                  0 if init_rows is None else len(init_rows), totals.ctypes.data,
                                   act_gen.ctypes.data, site_gen.ctypes.data, viol_counts.ctypes.data, msg, len(msg))
         if rc != 0:
             raise AuditError(f"{msg.value.decode()}  [{self.name}]")
@@ -273,10 +279,12 @@ def copy_parents(ck, first: int, count: int) -> np.ndarray:
     return buf
 
 
-def audit_checker(ck, levels: list[int], distinct: int, *, check_deadlock: bool | None = None, audit: AuditLib | None = None) -> dict:
+def audit_checker(ck, levels: list[int], distinct: int, *, check_deadlock: bool | None = None, audit: AuditLib | None = None,
+                  init_rows: np.ndarray | None = None) -> dict:
     """Audit the store of a Checker after a run: `levels` are the widths of the levels the run expanded (RunResult /
     ShardedResult .levels), `distinct` the stored states; the states past the expanded levels are the queue.  The
-    report holds the audit's totals and pick, the store and the run's kmc_violation_record (None without a violation)."""
+    report holds the audit's totals and pick, the store and the run's kmc_violation_record (None without a violation).
+    `init_rows` (see AuditLib.check_store) are the generated initial states of a device Init too large to enumerate."""
     a = audit or AuditLib.for_built_model(ck.meta["name"])
     if a.digest != ck.meta["digest"]:
         raise AuditError(f"digest: the audit's model.h ({a.digest}) is not the loaded library's ({ck.meta['digest']})")
@@ -286,7 +294,7 @@ def audit_checker(ck, levels: list[int], distinct: int, *, check_deadlock: bool 
     if distinct > sum(widths):
         widths.append(distinct - sum(widths))
     cd = a.check_deadlock if check_deadlock is None else check_deadlock
-    found = a.check_store(states, parents, widths, len(levels), check_deadlock=cd)
+    found = a.check_store(states, parents, widths, len(levels), check_deadlock=cd, init_rows=init_rows)
     record = ck.violation_record() if ck.violation() else None
     want = compare(a, found, stats=ck.stats(), coverage=ck.coverage(), parents=parents, violation=ck.violation(),
                    record=record, invariants=ck.meta["invariants"])
