@@ -194,6 +194,27 @@ int kmc_copy_states(const kmc_ctx* ctx, uint64_t first, uint64_t count, uint64_t
 /* parent words of the same range: bits 0..39 store index, 40..47 owner rank of the parent,
  * 56..63 action id; low 48 bits all ones = initial state (TLC's trace file)                 */
 int kmc_copy_parents(const kmc_ctx* ctx, uint64_t first, uint64_t count, uint64_t* buf);
+/* One transition of the state graph (kmc_edges): `src` is the global store index of the source state, `src_fp` and
+ * `dst_fp` the set-identity fingerprints of source and successor (state_fp: under SYMMETRY that of the orbit, the
+ * fingerprint kmc_violation reports), `action` the action id of model.json.                                          */
+typedef struct {
+  uint64_t src;
+  uint64_t src_fp;
+  uint64_t dst_fp;
+  uint32_t action;
+  uint32_t pad;
+} kmc_edge_t;
+/* Every transition out of the stored states [first, first+count) of the last kmc_run (TLC -dump dot): each successor
+ * the lowered Next generates and the CONSTRAINT keeps, duplicates and self-loops included, in no particular order.  The
+ * states are expanded again on the GPU (the non-fused expand kernel, then k_edges), in chunks that fit the candidate
+ * buffer; spilled states are staged from host memory.  The run is left exactly as it was: stats, coverage, violations,
+ * reports and the store.  Up to cap edges are written, *n receives the full count.  One GPU only: KMC_E_BADARG on a
+ * "gpus" > 1 or world > 1 context; KMC_E_STATE before a kmc_run; KMC_E_LAYOUT_OVERFLOW when a successor of the range
+ * does not fit the layout (the unexpanded last level of a stopped run can hold such a state).                        */
+int kmc_edges(kmc_ctx* ctx, uint64_t first, uint64_t count, kmc_edge_t* out, size_t cap, size_t* n);
+/* out[i] = set-identity fingerprint (as kmc_edge_t.src_fp) of stored state first + i, computed on the host; the
+ * same conditions as kmc_edges.                                                                                        */
+int kmc_fingerprints(kmc_ctx* ctx, uint64_t first, uint64_t count, uint64_t* out);
 /* this rank's offending state (packed words) and its parent word -- the starting point of a trace
  * walk that crosses ranks (a multi-rank driver follows parent words through kmc_copy_*)      */
 int kmc_violation_record(const kmc_ctx* ctx, uint64_t* words, size_t cap_words, uint64_t* parent_word);

@@ -23,6 +23,8 @@
 //                   k_invariant_report then passes a level's violators through record_invariants: violators
 //                   per invariant, and a second ring that holds the violators of invariants not reported
 //                   yet, so that every invariant gets its own first level and counterexample.
+//   k_edges (K5)    after a run (kmc_edges, TLC -dump dot): the candidate rows of a non-fused K1 over stored states
+//                   turned into compacted edge rows (source index, source and successor fingerprints, action).
 //
 // DESIGN.md sections 3-4 give the layout, the kernels and their measurements.
 //
@@ -1040,6 +1042,45 @@ __global__ void __launch_bounds__(256) k_insert(Params p, const uint64_t* rows, 
     if (probes) atomicAdd(&p.ctr->probes, (unsigned long long)probes);
     if (oom) atomicAdd(&p.ctr->out_of_model, (unsigned long long)oom);
     if (failed) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)failed);
+  }
+}
+
+// ----------------------------------------------------------------------------------------
+// K5: the transitions of a chunk of stored states (kmc_edges).  One thread per candidate row of a non-fused expand:
+// rows a CONSTRAINT discards are dropped, and every other row becomes an edge -- the source's global store index and
+// the set-identity fingerprints (state_fp) of source and successor, the source read back through the row's parent
+// index.  The source states lie at srcs[(parent index & src_mask) * W] and their global index is parent index +
+// src_offset (the device store in place, or a staging copy of spilled states).  A warp ballot compacts the edges.
+// ----------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_edges(const uint64_t* rows, const unsigned long long* n_ptr, const uint64_t* srcs,
+                                                uint64_t src_mask, uint64_t src_offset, uint64_t n_cap,
+                                                kmc_edge_t* out, unsigned long long* out_n) {
+  const uint64_t n = min((uint64_t)*n_ptr, n_cap);
+  const uint64_t n_round = (n + 31) & ~31ull;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const unsigned lane = lane_id();
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+    State s;
+    uint64_t meta;
+    load_row(s, meta, rows, i, i < n);
+    const bool keep = i < n && ((M::NUM_CONSTRAINTS == 0) || M::in_model(s));
+    kmc_edge_t e{};
+    if (keep) {
+      const uint64_t local = meta & IDX_MASK;
+      State src;
+      load_state(src, srcs + (local & src_mask) * W);
+      e.src = local + src_offset;
+      e.src_fp = state_fp(src);
+      e.dst_fp = state_fp(s);
+      e.action = (uint32_t)(meta >> 56);
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, keep);
+    if (m == 0) continue;
+    const int leader = __ffs(m) - 1;
+    unsigned long long base = 0;
+    if ((int)lane == leader) base = atomicAdd(out_n, (unsigned long long)__popc(m));
+    base = __shfl_sync(0xffffffffu, base, leader);
+    if (keep) out[base + __popc(m & ((1u << lane) - 1))] = e;
   }
 }
 
@@ -2170,6 +2211,16 @@ static int launch_invariants(Engine& E, uint64_t first, uint64_t count_bound) {
 
 // fused (kmc_run, one rank): the kernel inserts the successors itself; otherwise they go to the candidate buffer
 // (or the owners' inboxes) for k_insert / k_insert_inbox.  cand_bound (set_spill): a smaller bound on the chunk's successors.
+// the expand kernel's grid for `count` states; small levels get smaller tiles so that every SM still gets one (a tile
+// is a multiple of 32 states)
+static int expand_grid(const Engine& E, uint64_t count, unsigned* tile_states) {
+  const uint64_t ctas = (uint64_t)E.sms;
+  uint64_t per_cta = (count + ctas - 1) / ctas;
+  *tile_states = (unsigned)std::min<uint64_t>((uint64_t)TILE, std::max<uint64_t>(32, (per_cta + 31) & ~31ull));
+  uint64_t tiles = (count + *tile_states - 1) / *tile_states;
+  return (int)std::min<uint64_t>(tiles, ctas);
+}
+
 static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = false, bool fused = false, uint64_t cand_bound = 0) {
   Params p = E.params();
   p.p2p = p2p ? 1 : 0;
@@ -2177,12 +2228,8 @@ static int launch_expand(Engine& E, uint64_t first, uint64_t count, bool p2p = f
   if (cand_bound) p.region_rows = cand_bound;
   if (count == 0) return KMC_OK;
   TimedLaunch t(E, 0);
-  // small levels: smaller tiles so that every SM still gets one (a tile is a multiple of 32 states)
-  const uint64_t ctas = (uint64_t)E.sms;
-  uint64_t per_cta = (count + ctas - 1) / ctas;
-  unsigned tile_states = (unsigned)std::min<uint64_t>((uint64_t)TILE, std::max<uint64_t>(32, (per_cta + 31) & ~31ull));
-  uint64_t tiles = (count + tile_states - 1) / tile_states;
-  int grid = (int)std::min<uint64_t>(tiles, ctas);
+  unsigned tile_states;
+  const int grid = expand_grid(E, count, &tile_states);
   k_expand<<<grid, EXPAND_BLOCK, EXPAND_SMEM_BYTES, E.stream>>>(p, first, count, tile_states);
   CK(cudaGetLastError());
   return KMC_OK;
@@ -2241,6 +2288,84 @@ static int spill_below(Engine& E, uint64_t level_first) {
   if (rc) return rc;
   E.store_base = level_first;
   return KMC_OK;
+}
+
+// ---- kmc_edges: the transitions out of stored states -------------------------------------------------------------
+// The states [first, first + count) are expanded again, chunk by chunk, by the non-fused expand kernel into the
+// candidate buffer, and k_edges turns its rows into edges.  Nothing of the run changes: both kernels count into scratch
+// counters, deadlocks are not recorded (check_deadlock = 0) and nothing is inserted.  The candidate buffer (under
+// set_spill only its scratch part: the filter's marks lie behind it) is cut into the candidate rows, the edge rows and
+// a staging area for spilled states.  A chunk holds at most as many states as their MAX_FANOUT successors each fill, so
+// neither kind of row can overflow.  Spilled states (below store_base) are read through read_range and copied to the
+// staging area; the others are expanded in place, a chunk never crossing the ring's wrap.
+static constexpr int EDGE_WORDS = sizeof(kmc_edge_t) / 8;
+static_assert(sizeof(kmc_edge_t) == 32, "kmc_edge_t is four 64-bit words");
+
+struct EdgeScratch {
+  DevCounters ctr;
+  unsigned long long edges;
+};
+
+static int edges_chunks(Engine& E, EdgeScratch* d, uint64_t first, uint64_t count, kmc_edge_t* out, size_t cap,
+                        size_t* n) {
+  const uint64_t F = std::max<uint64_t>(1, (uint64_t)M::MAX_FANOUT);
+  const uint64_t words = E.set_spill ? set_scratch_words(E) : E.region_rows * ROW;
+  const uint64_t chunk = words > 1 ? (words - 1) / (F * (ROW + EDGE_WORDS) + W) : 0;      // (- 1: the staging alignment)
+  if (chunk == 0) {
+    E.last_error = "kmc_edges: the candidate buffer cannot hold one state's successors and their edges (raise cand_bytes)";
+    return KMC_E_BADARG;
+  }
+  uint64_t* rows = E.cand;
+  kmc_edge_t* edges = reinterpret_cast<kmc_edge_t*>(E.cand + chunk * F * ROW);
+  uint64_t* staging = E.cand + ((chunk * F * (ROW + EDGE_WORDS) + 1) & ~1ull);          // 16-byte aligned tile loads
+  Params p = E.params();
+  p.ctr = &d->ctr;
+  p.check_deadlock = 0;
+  p.region_rows = chunk * F;
+  std::vector<uint64_t> host;
+  size_t total = 0;
+  for (uint64_t g = first, end = first + count, slot, cnt; g < end; g += cnt) {
+    Params q = p;
+    uint64_t start = g, offset = 0;
+    if (g < E.store_base) {
+      cnt = std::min({chunk, E.store_base - g, end - g});
+      host.resize(cnt * W);
+      if (int rc = read_range(E, g, cnt, host.data(), nullptr)) return rc;
+      CK(cudaMemcpyAsync(staging, host.data(), cnt * W * 8, cudaMemcpyHostToDevice, E.stream));
+      q.store = staging;
+      q.store_mask = ~0ull;
+      start = 0;
+      offset = g;
+    } else {
+      cnt = std::min(chunk, ring_run(E, g, end, &slot));
+    }
+    CK(cudaMemsetAsync(d, 0, sizeof(EdgeScratch), E.stream));
+    unsigned tile_states;
+    const int grid = expand_grid(E, cnt, &tile_states);
+    k_expand<<<grid, EXPAND_BLOCK, EXPAND_SMEM_BYTES, E.stream>>>(q, start, cnt, tile_states);
+    k_edges<<<grid_for(E, cnt * F, 256, 8), 256, 0, E.stream>>>(rows, &d->ctr.cand_count[0], q.store, q.store_mask, offset,
+                                                                p.region_rows, edges, &d->edges);
+    CK(cudaGetLastError());
+    unsigned long long fail = 0, k = 0;
+    CK(cudaMemcpyAsync(&fail, &d->ctr.fail, 8, cudaMemcpyDeviceToHost, E.stream));
+    CK(cudaMemcpyAsync(&k, &d->edges, 8, cudaMemcpyDeviceToHost, E.stream));
+    CK(cudaStreamSynchronize(E.stream));
+    // a successor that does not fit the layout (the unexpanded last level of a stopped run can hold one): an error
+    if (fail) return fail_to_error(fail);
+    if (total < cap) CK(cudaMemcpy(out + total, edges, std::min<uint64_t>(k, cap - total) * sizeof(kmc_edge_t),
+                                   cudaMemcpyDeviceToHost));
+    total += k;
+  }
+  *n = total;
+  return KMC_OK;
+}
+
+static int engine_edges(Engine& E, uint64_t first, uint64_t count, kmc_edge_t* out, size_t cap, size_t* n) {
+  EdgeScratch* d = nullptr;
+  CK(cudaMalloc(&d, sizeof(EdgeScratch)));
+  const int rc = edges_chunks(E, d, first, count, out, cap, n);
+  cudaFree(d);
+  return rc;
 }
 
 // ---- checkpoint / recover (TLC -checkpoint / -recover): written at a level boundary -------------------------------
@@ -2902,6 +3027,45 @@ int kmcm_copy_parents(const kmcm_ctx* c, uint64_t first, uint64_t count, uint64_
 }
 int kmcm_copy_states(const kmcm_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) {
   return copy_store(c, first, count, buf, nullptr);
+}
+
+// kmc_edges and kmc_fingerprints read the store a kmc_run left on one GPU
+static int stored_range(kmcm_ctx* c, uint64_t first, uint64_t count) {
+  if (!c->ranks.empty() || E.world > 1) {
+    E.last_error = "kmc_edges / kmc_fingerprints read the store of a one-GPU kmc_run: no \"gpus\" > 1, no world > 1";
+    return KMC_E_BADARG;
+  }
+  if (!E.ran) return KMC_E_STATE;
+  if (first + count < first || first + count > E.stats.distinct) {
+    E.last_error = "kmc_edges / kmc_fingerprints: the range reaches past the stored states";
+    return KMC_E_BADARG;
+  }
+  CK(cudaSetDevice(E.device));
+  return KMC_OK;
+}
+
+int kmcm_edges(kmcm_ctx* c, uint64_t first, uint64_t count, kmc_edge_t* out, size_t cap, size_t* n) {
+  if (!c || !n || (cap && !out)) return KMC_E_BADARG;
+  if (int rc = stored_range(c, first, count)) return rc;
+  return engine_edges(E, first, count, out, cap, n);
+}
+
+// host side: state_fp is a host function too, and a fingerprint per stored state is what a graph writer needs once
+int kmcm_fingerprints(kmcm_ctx* c, uint64_t first, uint64_t count, uint64_t* out) {
+  if (!c || (count && !out)) return KMC_E_BADARG;
+  if (int rc = stored_range(c, first, count)) return rc;
+  std::vector<uint64_t> buf;
+  for (uint64_t g = first, end = first + count, m; g < end; g += m) {
+    m = std::min<uint64_t>(end - g, 1 << 20);
+    buf.resize(m * W);
+    if (int rc = read_range(E, g, m, buf.data(), nullptr)) return rc;
+    for (uint64_t i = 0; i < m; ++i) {
+      State s;
+      memcpy(s.w, buf.data() + i * W, sizeof(s.w));
+      out[g - first + i] = state_fp(s);
+    }
+  }
+  return KMC_OK;
 }
 
 const char* kmcm_strerror(const kmcm_ctx* c, int code) {

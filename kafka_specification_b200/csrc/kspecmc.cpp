@@ -32,6 +32,8 @@ struct kmc_ctx {
   int (*trace_state)(const kmcm_ctx*, uint32_t, uint64_t*, size_t, uint32_t*) = nullptr;
   int (*copy_states)(const kmcm_ctx*, uint64_t, uint64_t, uint64_t*) = nullptr;
   int (*copy_parents)(const kmcm_ctx*, uint64_t, uint64_t, uint64_t*) = nullptr;
+  int (*edges)(kmcm_ctx*, uint64_t, uint64_t, kmc_edge_t*, size_t, size_t*) = nullptr;
+  int (*fingerprints)(kmcm_ctx*, uint64_t, uint64_t, uint64_t*) = nullptr;
   int (*violation_record)(const kmcm_ctx*, uint64_t*, size_t, uint64_t*) = nullptr;
   int (*invariant_reports)(const kmcm_ctx*, kmc_invariant_report_t*, size_t, size_t*, int32_t*) = nullptr;
   int (*invariant_trace_state)(const kmcm_ctx*, int32_t, uint32_t, uint64_t*, size_t, uint32_t*) = nullptr;
@@ -88,6 +90,7 @@ int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out) {
             bind(c, c->violation, "kmcm_violation") &&
             bind(c, c->trace_state, "kmcm_trace_state") && bind(c, c->copy_states, "kmcm_copy_states") &&
             bind(c, c->copy_parents, "kmcm_copy_parents") && bind(c, c->violation_record, "kmcm_violation_record") &&
+            bind(c, c->edges, "kmcm_edges") && bind(c, c->fingerprints, "kmcm_fingerprints") &&
             bind(c, c->invariant_reports, "kmcm_invariant_reports") &&
             bind(c, c->invariant_trace_state, "kmcm_invariant_trace_state") &&
             bind(c, c->strerror_, "kmcm_strerror") && bind(c, c->fpset_put, "kmcm_fpset_put") &&
@@ -136,6 +139,10 @@ int kmc_violation(const kmc_ctx* c, kmc_violation_t* out) { FWD(violation, out);
 int kmc_trace_state(const kmc_ctx* c, uint32_t i, uint64_t* buf, size_t cap, uint32_t* a) { FWD(trace_state, i, buf, cap, a); }
 int kmc_copy_states(const kmc_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) { FWD(copy_states, first, count, buf); }
 int kmc_copy_parents(const kmc_ctx* c, uint64_t first, uint64_t count, uint64_t* buf) { FWD(copy_parents, first, count, buf); }
+int kmc_edges(kmc_ctx* c, uint64_t first, uint64_t count, kmc_edge_t* out, size_t cap, size_t* n) {
+  FWD(edges, first, count, out, cap, n);
+}
+int kmc_fingerprints(kmc_ctx* c, uint64_t first, uint64_t count, uint64_t* out) { FWD(fingerprints, first, count, out); }
 int kmc_violation_record(const kmc_ctx* c, uint64_t* words, size_t cap, uint64_t* meta) { FWD(violation_record, words, cap, meta); }
 int kmc_invariant_reports(const kmc_ctx* c, kmc_invariant_report_t* out, size_t cap, size_t* n, int32_t* complete) {
   FWD(invariant_reports, out, cap, n, complete);

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes
 import json
 import os
+import time
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -67,6 +68,11 @@ class ModelInfo(ctypes.Structure):
                 ("name", ctypes.c_char * 128), ("digest", ctypes.c_char * 32), ("init_candidates", ctypes.c_uint64)]
 
 
+# kmc_edge_t as a numpy record: Checker.edges returns arrays of it, which kmc_edges fills in place
+EDGE_DTYPE = np.dtype([("src", np.uint64), ("src_fp", np.uint64), ("dst_fp", np.uint64), ("action", np.uint32),
+                       ("pad", np.uint32)])
+
+
 class ShardBuffers(ctypes.Structure):
     _fields_ = [("cand", ctypes.c_void_p), ("region_rows", ctypes.c_uint64), ("cand_counts", ctypes.c_void_p),
                 ("recv", ctypes.c_void_p), ("recv_rows_cap", ctypes.c_uint64), ("row_words", ctypes.c_int32)]
@@ -101,6 +107,8 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.kmc_copy_states.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp]
     lib.kmc_copy_parents.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp]
     lib.kmc_violation_record.argtypes = [vp, u64p, ctypes.c_size_t, u64p]
+    lib.kmc_edges.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
+    lib.kmc_fingerprints.argtypes = [vp, ctypes.c_uint64, ctypes.c_uint64, vp]
     lib.kmc_invariant_reports.argtypes = [vp, ctypes.POINTER(InvariantReport), ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t),
                                           ctypes.POINTER(ctypes.c_int32)]
     lib.kmc_invariant_trace_state.argtypes = [vp, ctypes.c_int32, ctypes.c_uint32, u64p, ctypes.c_size_t,
@@ -129,7 +137,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.kmc_shard_inbox_ptr.argtypes = [vp, ctypes.POINTER(vp)]
     lib.kmc_shard_open_peers_direct.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.c_uint32]
     for fn in ("kmc_create", "kmc_model_info", "kmc_run", "kmc_stats", "kmc_level_widths", "kmc_action_counts", "kmc_coverage",
-               "kmc_violation", "kmc_trace_state", "kmc_copy_states", "kmc_copy_parents", "kmc_violation_record", "kmc_invariant_reports", "kmc_invariant_trace_state", "kmc_fpset_put", "kmc_fpset_contains",
+               "kmc_violation", "kmc_trace_state", "kmc_copy_states", "kmc_copy_parents", "kmc_violation_record", "kmc_edges", "kmc_fingerprints", "kmc_invariant_reports", "kmc_invariant_trace_state", "kmc_fpset_put", "kmc_fpset_contains",
                "kmc_fpset_size", "kmc_shard_begin", "kmc_shard_buffers", "kmc_shard_seed_init", "kmc_shard_expand",
                "kmc_shard_counts", "kmc_shard_reset_cand", "kmc_shard_insert", "kmc_shard_level_done", "kmc_shard_sync",
                "kmc_shard_ipc_handle", "kmc_shard_open_peers", "kmc_shard_seed_p2p", "kmc_shard_expand_p2p",
@@ -393,6 +401,85 @@ class Checker:
         if count:
             self._check(self.lib.kmc_copy_states(self.ctx, first, count, buf.ctypes.data))
         return buf
+
+    # -- the state set and the state graph (TLC -dump) ------------------------
+    def level_ranges(self) -> list[tuple[int, int]]:
+        """(first, count) of every BFS level in the store; the last one is the queue when the run stopped early."""
+        out, first = [], 0
+        for w in self.level_widths():
+            out.append((first, w))
+            first += w
+        distinct = self.stats()["distinct"]
+        if distinct > first:
+            out.append((first, distinct - first))
+        return out
+
+    def edges(self, first: int, count: int, chunk: int = 1 << 20) -> np.ndarray:
+        """Every transition out of the stored states [first, first+count) as an ``EDGE_DTYPE`` array: the successors the
+        lowered Next generates and the CONSTRAINT keeps, duplicates and self-loops included, in no particular order
+        (kmc_edges, enumerated on the GPU; the run's results are left as they were).  The states go to kmc_edges ``chunk``
+        at a time; a chunk whose edges outgrow the buffer (sized for min(max_fanout, 8) per state, then for the largest
+        count seen) is asked for again with room for all of them."""
+        parts, n = [], ctypes.c_size_t()
+        per_state = max(1, min(self.info.max_fanout, 8))
+        for off in range(first, first + count, chunk):
+            m = min(chunk, first + count - off)
+            cap = m * per_state
+            while True:
+                buf = np.empty(cap, dtype=EDGE_DTYPE)
+                self._check(self.lib.kmc_edges(self.ctx, off, m, buf.ctypes.data, cap, ctypes.byref(n)))
+                if n.value <= cap:
+                    break
+                cap = n.value
+            per_state = max(per_state, -(-n.value // m))
+            parts.append(buf[:n.value])
+        return np.concatenate(parts) if parts else np.empty(0, dtype=EDGE_DTYPE)
+
+    def fingerprints(self, first: int, count: int) -> np.ndarray:
+        """Set-identity fingerprint of each stored state [first, first+count) (``edges()``'s ``src_fp``)."""
+        out = np.empty(count, dtype=np.uint64)
+        if count:
+            self._check(self.lib.kmc_fingerprints(self.ctx, first, count, out.ctypes.data))
+        return out
+
+    def dump_states(self, path: str, batch: int = 1 << 20) -> dict:
+        """Writes every stored state to ``path`` as TLC's ``-dump`` does (``State k:`` and the state's text, see
+        ``dump.py``), level by level; within a level the states are ordered by their packed words, so that the file does
+        not depend on which insert won (identical across runs, ``spill`` and ``set_spill`` without SYMMETRY).  Returns
+        the states written and the seconds spent decoding and writing."""
+        from . import dump
+        t = {"states": 0, "decode_s": 0.0, "write_s": 0.0}
+        with open(path, "w") as f:
+            for first, count in self.level_ranges():
+                rows = dump.sorted_rows(self.copy_states(first, count))
+                for b in range(0, count, batch):
+                    t0 = time.perf_counter()
+                    texts = self.decoder.texts(rows[b:b + batch])
+                    t1 = time.perf_counter()
+                    t["states"] += dump.write_states(f, texts, t["states"] + 1)
+                    t["write_s"] += time.perf_counter() - t1
+                    t["decode_s"] += t1 - t0
+        return t
+
+    def dump_dot(self, path: str, actionlabels: bool = False, colorize: bool = False) -> dict:
+        """Writes the state graph to ``path`` in TLC's DotStateWriter layout (``dump.write_dot``): a node per stored
+        state, initial states filled, and one edge per distinct (source, successor, action) out of the expanded states
+        (``distinct - queue``: a stopped run shows the graph explored so far)."""
+        from . import dump
+        st = self.stats()
+        ranges = self.level_ranges()
+        nodes_fp, texts = [], []
+        for first, count in ranges:
+            rows = self.copy_states(first, count)
+            order = dump.row_order(rows)
+            nodes_fp.append(self.fingerprints(first, count)[order])
+            texts += self.decoder.texts(rows[order])
+        n_init = ranges[0][1] if ranges else 0
+        edges = self.edges(0, st["distinct"] - st["queue"])
+        actions = [a["name"] for a in self.meta["actions"]]
+        fps = np.concatenate(nodes_fp) if nodes_fp else np.empty(0, dtype=np.uint64)
+        with open(path, "w") as f:
+            return dump.write_dot(f, fps, texts, n_init, edges, actions, actionlabels=actionlabels, colorize=colorize)
 
     # -- fingerprint set alone (FPSet.put / contains / size) -----------------
     def fpset_put(self, fps: np.ndarray) -> np.ndarray:

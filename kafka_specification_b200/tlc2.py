@@ -2,7 +2,8 @@
 
     python -m kafka_specification_b200.tlc2 [-config F.cfg] [-workers N|auto] [-deadlock] [-continue]
                                              [-fpbits N] [-maxstates N] [-I dir] [-metadir d] [-checkpoint MIN]
-                                             [-recover DIR] [-spill] [-setspill] [-coverage N] [-tool] SPEC
+                                             [-recover DIR] [-spill] [-setspill] [-coverage N] [-tool]
+                                             [-dump FILE | -dump dot[,actionlabels][,colorize][,snapshot] FILE] SPEC
 
 ``SPEC`` is a module name or a path to ``SPEC.tla``; modules it EXTENDS / INSTANCEs are resolved
 from the same directory (and ``-I`` directories), like TLC does.  The spec and its ``.cfg`` are
@@ -20,6 +21,9 @@ level, cfg index), each with the counterexample that ends in the smallest-finger
 block is the one a run without ``-continue`` prints.  TLC under ``-continue`` prints a trace for every violating state
 it meets (as far as its published behaviour goes: TLC cannot be run here to compare); here it is one per invariant.
 A deadlock found on the way keeps its block and its exit status, ahead of the invariant blocks.
+``-dump FILE`` writes every reachable state to ``FILE.dump``; ``-dump dot,... FILE`` writes the state graph, its
+transitions enumerated on the GPU, to ``FILE.dot`` (one GPU; see ``dump.py`` for the layouts and how they differ from
+TLC's).  The file is written once, at the end of the run, after a violation too; ``snapshot`` is accepted and ignored.
 
 Exit status follows TLC: 0 no error, 12 safety (invariant) violation, 11 deadlock,
 10 assumption failure, 150 spec/config error, 1 runtime failure (no GPU, table full, ...).
@@ -39,6 +43,7 @@ from .frontend.cfg import CfgError
 from .frontend.modules import ModuleError
 from .frontend.tla_lexer import TlaSyntaxError
 from .lower.svals import LowerError
+from .dump import split_dump_args
 from .runtime import Checker, KmcError
 
 EXIT_OK, EXIT_VIOLATION_ASSUMPTION, EXIT_VIOLATION_DEADLOCK, EXIT_VIOLATION_SAFETY, EXIT_ERROR_SPEC = 0, 10, 11, 12, 150
@@ -159,8 +164,20 @@ def error_messages(violation: dict | None, trace: list[dict], reports: list[dict
     return out, code
 
 
+def write_dump(ck: Checker, req) -> None:
+    if req.dot:
+        ck.dump_dot(req.path, actionlabels=req.actionlabels, colorize=req.colorize)
+    else:
+        ck.dump_states(req.path)
+
+
 def main(argv=None) -> int:
-    a = parse_args(argv if argv is not None else sys.argv[1:])
+    try:
+        argv, dump_req = split_dump_args(list(argv if argv is not None else sys.argv[1:]))
+    except ValueError as e:
+        print(f"Error: {e}")
+        return EXIT_ERROR_SPEC
+    a = parse_args(argv)
     spec_path = a.spec[:-4] if a.spec.endswith(".tla") else a.spec
     spec_dir = os.path.dirname(os.path.abspath(spec_path)) if os.path.dirname(spec_path) else os.getcwd()
     module = os.path.basename(spec_path)
@@ -246,6 +263,12 @@ def main(argv=None) -> int:
         n_init = r.levels[0] if r.levels else r.distinct
     msg("init_done", f"Finished computing initial states: {n_init} distinct state{'s' if n_init != 1 else ''} generated.")
     blocks, exit_code = error_messages(r.violation, r.trace, r.invariant_violations)
+    if dump_req is not None:
+        try:
+            write_dump(ck, dump_req)
+        except (KmcError, OSError) as e:
+            msg("general", f"Error: cannot write {dump_req.path}: {e}", 1)
+            return 1
     for kind, text, cls in blocks:
         msg(kind, text, cls)
     if not blocks:
