@@ -61,7 +61,8 @@ enum {
   KMC_E_STATE = -8,           /* call sequence error (e.g. trace before run)             */
   KMC_E_NO_GPU = -9,          /* no CUDA device: there is deliberately no CPU fallback   */
   KMC_E_CAND_FULL = -10,      /* candidate buffer overflow (raise cand_bytes / fanout_bound) */
-  KMC_E_PEER_TIMEOUT = -11    /* multi-GPU: a peer rank never reached a device-side synchronisation point */
+  KMC_E_PEER_TIMEOUT = -11,   /* multi-GPU: a peer rank never reached a device-side synchronisation point */
+  KMC_E_SET_TIMEOUT = -12     /* "exact_set": a claimed slot of the set was not published within its bounded wait */
 };
 
 /* result kinds (kmc_violation_t.kind); a driver maps them to TLC's exit codes 0/12/11 */
@@ -87,7 +88,8 @@ typedef struct {
   uint64_t max_states;      /* state-store capacity                                       */
   uint64_t complete;        /* 1 if the search ran to an empty queue                      */
   double gpu_ms_invariant;  /* sum over invariant-kernel launches (counted in launches_other) */
-  uint64_t slot_bytes;      /* 8: 64-bit fingerprints (one-word states); 16: 128-bit keys (the state itself when it fits) */
+  uint64_t slot_bytes;      /* 8: 64-bit fingerprints (one-word states); 16: 128-bit keys (the state itself when it fits);
+                               "exact_set" on a hashed model: 16 (one word), 32 (two or three words), 64 (four to seven) */
   uint64_t set_flushes;     /* "set_spill": times the table's keys moved to host memory                */
   uint64_t set_host_keys;   /* "set_spill": keys in host memory (each distinct state's key at most once) */
   uint64_t set_filtered;    /* "set_spill": appended states removed because their key was in host memory */
@@ -125,7 +127,8 @@ typedef struct {
   int32_t num_init;
   int32_t max_fanout;       /* static bound on successors per state                       */
   int32_t check_deadlock;
-  int32_t exact;            /* 1: the set key is a bijection of the state (<= 63 bits, or two words stored as a 128-bit key) */
+  int32_t exact;            /* 1: the set key is a bijection of the state (<= 63 bits, or two words stored as a 128-bit key),
+                               or the context was created with "exact_set" (the key is then the packed state) */
   char name[128];
   char digest[32];
   uint64_t init_candidates;  /* device Init: candidate assignments over all branches (num_init is then 0); 0 for a table */
@@ -151,6 +154,15 @@ typedef struct {
  *   whose key is in host memory are removed before each move and at each level end, so the results are those of a run
  *   with a table large enough.  With "spill" host memory bounds the run; about slot_bytes + 8 * words + 8 bytes per
  *   state, and KMC_E_OOM when it runs out.  A set_spill context refuses "gpus" > 1, world > 1, the kmc_shard_* calls and kmc_fpset_*: KMC_E_BADARG).
+ * "exact_set":false (an extension, one GPU only: the fingerprint set's key is the packed state itself -- under SYMMETRY
+ *   its orbit's canonical form -- so that no two distinct states can share a key and "no violation" is exact on every
+ *   model, not only on those whose key is a bijection already (kmc_model_info.exact = 1 without the option; there the
+ *   option is accepted and changes nothing).  A slot is a header word and the state's words: slot_bytes 16 at one word,
+ *   32 at two or three, 64 at four to seven, so the same table_log2 takes 1x, 2x or 4x the memory of the 16-byte form
+ *   and the default sizing gives a table of fewer slots.  The 64-bit fingerprint still picks the bucket, orders the
+ *   counterexamples and names -dump dot nodes.  It combines with "spill", "set_spill" (the keys in host memory are the
+ *   states' words) and "recover".  An exact_set context refuses "gpus" > 1, world > 1, the kmc_shard_* calls and
+ *   kmc_fpset_* (a 64-bit fingerprint is not a key of this set): KMC_E_BADARG with a message.
  * Unknown keys are ignored.  */
 int kmc_create(const char* model_lib, const char* options_json, kmc_ctx** out);
 void kmc_destroy(kmc_ctx* ctx);

@@ -69,6 +69,7 @@ static_assert(M::NUM_ACTIONS <= 255, "the parent word holds the action id in 8 b
 #define KMC_FAIL_STORE_FULL 3
 #define KMC_FAIL_CAND_FULL 4
 #define KMC_FAIL_PEER_TIMEOUT 5
+#define KMC_FAIL_SET_TIMEOUT 6
 
 // ----------------------------------------------------------------------------------------
 // fingerprints
@@ -89,6 +90,7 @@ __host__ __device__ __forceinline__ uint64_t fmix64(uint64_t x) {
 //   wider models                : a 128-bit fingerprint (two independent 64-bit chains) in 16-byte slots;
 //                                 collision probability ~ n^2 / 2^129 (TLC's FP64 contract squared)
 // The 64-bit fingerprint also picks the bucket and the owner rank and orders counterexamples.
+// The option "exact_set" makes the hashed forms exact too: the key is then the packed state (see XSLOT_WORDS).
 static constexpr bool KEY128 = (W >= 2);
 static constexpr bool EXACT_SET = EXACT64 || (W == 2 && !M::ALL_ONES_POSSIBLE);
 static constexpr int BUCKET_SLOTS = KEY128 ? 2 : 4;      // one 32 B sector per bucket
@@ -100,11 +102,20 @@ struct alignas(16) Key128 {
 __host__ __device__ __forceinline__ bool key_eq(const Key128& a, const Key128& b) { return a.lo == b.lo && a.hi == b.hi; }
 __host__ __device__ __forceinline__ bool key_empty(const Key128& a) { return (a.lo & a.hi) == ~0ull; }
 
+// KMC_TEST_FP_BITS (tests only, never in a default build): the hashed fingerprint keeps only its low bits and the hashed
+// 128-bit key none beyond them, so that distinct states collide and a set keyed by them visibly loses states.
+#ifdef KMC_TEST_FP_BITS
+static constexpr uint64_t TEST_FP_MASK = (1ull << KMC_TEST_FP_BITS) - 1, TEST_KEY_HI_MASK = 0;
+#else
+static constexpr uint64_t TEST_FP_MASK = ~0ull, TEST_KEY_HI_MASK = ~0ull;
+#endif
+
 __host__ __device__ __forceinline__ uint64_t fingerprint(const State& s) {
   if (EXACT64) return fmix64(s.w[0] + 1);
   uint64_t h = fmix64(s.w[0] + 0x9E3779B97F4A7C15ull);
 #pragma unroll
   for (int i = 1; i < W; ++i) h = fmix64(h ^ (s.w[i] + 0x9E3779B97F4A7C15ull * (uint64_t)(i + 1)));
+  h &= TEST_FP_MASK;
   return h ? h : 1;
 }
 __host__ __device__ __forceinline__ uint64_t fmix64b(uint64_t x) {     // a second, unrelated finaliser (splitmix64's)
@@ -125,7 +136,7 @@ __host__ __device__ __forceinline__ Key128 key_of(const State& s, uint64_t fp) {
 #pragma unroll
     for (int i = 1; i < W; ++i) h = fmix64b((h << 7 | h >> 57) ^ s.w[i]);
     k.lo = fp;
-    k.hi = h;
+    k.hi = h & TEST_KEY_HI_MASK;
     if (key_empty(k)) k.hi ^= 1;
   }
   return k;
@@ -156,6 +167,20 @@ __host__ __device__ __forceinline__ Ident state_ident(const State& s) {
   return id;
 }
 __host__ __device__ __forceinline__ uint64_t state_fp(const State& s) { return state_ident(s).fp; }
+
+// exact_set: the key is the packed state itself -- the orbit representative under SYMMETRY -- and fp is state_fp's.
+__host__ __device__ __noinline__ void canonical_xident(const State& s, State& key, uint64_t& fp) {
+  M::canonicalize(s, key);
+  fp = fingerprint(key);
+}
+__host__ __device__ __forceinline__ void state_xident(const State& s, State& key, uint64_t& fp) {
+  if (M::HAS_SYMMETRY) {
+    canonical_xident(s, key, fp);
+  } else {
+    key = s;
+    fp = fingerprint(s);
+  }
+}
 
 __host__ __device__ __forceinline__ uint32_t owner_of(uint64_t fp, uint32_t world) {
   return (uint32_t)(((fp >> 32) * (uint64_t)world) >> 32);
@@ -232,6 +257,7 @@ struct Params {
   // sound because every new index lies at or beyond the end of the level being expanded, and the
   // `idx - store_base < max_states` check of insert_row keeps a spilling ring from wrapping onto live states.
   uint32_t fused;
+  uint32_t exact;           // 1: the option "exact_set" on a model whose key is hashed (never set when EXACT_SET)
 };
 
 static constexpr int INBOX_HEADER = 8;
@@ -425,24 +451,147 @@ __device__ __forceinline__ long long set_contains(const void* table, uint64_t bu
   return -1;
 }
 
+// ---- exact_set: the key is the packed state (DESIGN.md section 4, "Identity of a state") ----------------------------
+// A slot is a header word and the W words of the key, padded to 16 B (W = 1: two slots per 32 B bucket), 32 B (W = 2, 3)
+// or 64 B (W = 4 .. 7: one bucket of two sectors).  Header: XEMPTY, then CLAIMED (tag = fp & ~3: the claimer is writing
+// the words), then PUBLISHED (tag | 1).  Neither can be all-ones (bit 0 clear; bit 1 clear), so the table's empty marker
+// is the all-ones fill of the 16-byte form.  A slot is claimed by one CAS on its header and never changes key.
+// XS_ON is `true` only where the option can do anything: models whose key is exact already compile no exact_set code.
+static constexpr bool XS_ON = !EXACT_SET;
+static constexpr int XSLOT_WORDS = W == 1 ? 2 : (W <= 3 ? 4 : 8);
+static constexpr int XBUCKET_SLOTS = W == 1 ? 2 : 1;
+static constexpr int XSLOT_BYTES = XSLOT_WORDS * 8;
+static constexpr int XPROBE_BUCKETS = 1024 / XBUCKET_SLOTS;     // the same 1024 slots as the 16-byte form's 512 buckets
+static constexpr uint64_t XEMPTY = ~0ull;
+static constexpr int XWAIT_ROUNDS = 1 << 20;                    // of >= 64 ns: a publish not seen in ~0.1 s fails the run
+
+__device__ __forceinline__ uint64_t* xslot_addr(const void* table, uint64_t b, int k) {
+  return const_cast<uint64_t*>(static_cast<const uint64_t*>(table)) + (b * XBUCKET_SLOTS + k) * XSLOT_WORDS;
+}
+// the first sector of bucket b: the header of each of its slots (v[k].x for W = 1, v[0].x otherwise)
+__device__ __forceinline__ Bucket ld_xbucket(const void* table, uint64_t b) {
+  Bucket k;
+  const char* base = reinterpret_cast<const char*>(xslot_addr(table, b, 0));
+#pragma unroll
+  for (int i = 0; i < BUCKET_LOADS; ++i) k.v[i] = ld_cg128(base + 16 * i);
+  return k;
+}
+__device__ __forceinline__ uint64_t xheader(const Bucket& bk, int k) { return W == 1 && k ? bk.v[1].x : bk.v[0].x; }
+__device__ __forceinline__ uint64_t ld_acquire64(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release64(uint64_t* p, uint64_t v) {
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ uint64_t ld_cg64(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(v) : "l"(p));
+  return v;
+}
+
+// A slot whose header carries the key's tag: 1 when it holds the key, 0 when another key, -2 when its claimer has not
+// published within XWAIT_ROUNDS.  The words are read after an acquire load that saw the header published, so they are
+// the claimer's words, never a half-written slot.
+__device__ __noinline__ int xslot_match(const uint64_t* slot, const State& key) {
+  uint64_t h = ld_acquire64(slot);
+  for (int i = 0; !(h & 1); ++i) {
+    if (i == XWAIT_ROUNDS) return -2;
+    __nanosleep(64);
+    h = ld_acquire64(slot);
+  }
+  bool eq = true;
+#pragma unroll
+  for (int w = 0; w < W; ++w) eq &= ld_cg64(slot + 1 + w) == key.w[w];
+  return eq ? 1 : 0;
+}
+
+// returns 1 = inserted (new), 0 = already present, -1 = table full, -2 = a publish was never seen.  `bk` = the first
+// bucket's headers, loaded by the caller ahead of time.  Every inserter of a key scans the same slots in the same order
+// and passes a slot only when it is verified to hold another key (a different tag, or the published words differ), so a
+// key occupies at most one slot; a stale header is harmless (the CAS decides, and a tag never changes).
+__device__ __forceinline__ int xset_insert(void* table, uint64_t bucket_mask, uint64_t fp, const State& key, Bucket bk,
+                                           unsigned& probes) {
+  const uint64_t tag = fp & ~3ull;
+  uint64_t b = bucket_of(fp, bucket_mask);
+  for (int attempt = 0; attempt < XPROBE_BUCKETS; ++attempt) {
+    ++probes;
+#pragma unroll
+    for (int k = 0; k < XBUCKET_SLOTS; ++k) {
+      uint64_t* slot = xslot_addr(table, b, k);
+      uint64_t h = attempt ? ld_cg64(slot) : xheader(bk, k);
+      if (h == XEMPTY) {
+        h = atomicCAS(reinterpret_cast<unsigned long long*>(slot), (unsigned long long)XEMPTY, (unsigned long long)tag);
+        if (h == XEMPTY) {
+#pragma unroll
+          for (int w = 0; w < W; ++w) slot[1 + w] = key.w[w];
+          st_release64(slot, tag | 1);        // the words are visible to whoever sees the header published
+          return 1;
+        }
+      }
+      if ((h & ~1ull) != tag) continue;       // another key
+      const int m = xslot_match(slot, key);
+      if (m) return m > 0 ? 0 : m;
+    }
+    b = (b + 1) & bucket_mask;
+  }
+  return -1;
+}
+
+// the slot that holds the key, or -1.  Only called while no insert runs (every claimed slot is published), and an
+// empty slot ends the probe: an inserter never passes one.
+__device__ __forceinline__ long long xset_contains(const void* table, uint64_t bucket_mask, uint64_t fp, const State& key) {
+  const uint64_t tag = fp & ~3ull;
+  uint64_t b = bucket_of(fp, bucket_mask);
+  for (int attempt = 0; attempt < XPROBE_BUCKETS; ++attempt) {
+#pragma unroll
+    for (int k = 0; k < XBUCKET_SLOTS; ++k) {
+      const uint64_t* slot = xslot_addr(table, b, k);
+      const uint64_t h = ld_cg64(slot);
+      if (h == XEMPTY) return -1;
+      if ((h & ~1ull) == tag && xslot_match(slot, key) > 0) return (long long)(b * XBUCKET_SLOTS + k);
+    }
+    b = (b + 1) & bucket_mask;
+  }
+  return -1;
+}
+
 // Warp-collective insert of one candidate row per lane (invalid lanes pass valid = false):
 // constraint check, identity, bucket probe + CAS, ballot/popc compaction of the winners into the
 // state store, parent link.
+// XS: the exact_set form, which carries the key (the packed state, canonical under SYMMETRY) instead of Ident::key.
+template <bool XS = false>
 struct Prefetched {
   Ident id;
   Bucket bk;
   bool inmodel;
 };
+template <>
+struct Prefetched<true> {
+  Ident id;
+  Bucket bk;
+  bool inmodel;
+  State key;
+};
 
 // first half of an insert: identity + issue the bucket loads (no dependent use yet)
-__device__ __forceinline__ Prefetched prefetch_row(const Params& p, const State& s, bool valid) {
-  Prefetched f;
+template <bool XS = false>
+__device__ __forceinline__ Prefetched<XS> prefetch_row(const Params& p, const State& s, bool valid) {
+  Prefetched<XS> f;
   f.id.fp = 0;
   f.id.key = Key128{0, 0};
 #pragma unroll
   for (int i = 0; i < BUCKET_LOADS; ++i) f.bk.v[i] = make_ulonglong2(0, 0);
   f.inmodel = false;
-  if (valid) {
+  if constexpr (XS) {
+    f.key = s;
+    if (valid) {
+      f.inmodel = (M::NUM_CONSTRAINTS == 0) || M::in_model(s);
+      state_xident(s, f.key, f.id.fp);
+      if (f.inmodel) f.bk = ld_xbucket(p.table, bucket_of(f.id.fp, p.bucket_mask));
+    }
+  } else if (valid) {
     f.inmodel = (M::NUM_CONSTRAINTS == 0) || M::in_model(s);
     f.id = state_ident(s);
     if (f.inmodel) f.bk = ld_bucket(p.table, bucket_of(f.id.fp, p.bucket_mask));
@@ -452,14 +601,20 @@ __device__ __forceinline__ Prefetched prefetch_row(const Params& p, const State&
 
 // CTA_ACTIONS: the new states per action go to this CTA's shared-memory counters at `act_smem` (u64 per action, the
 // fused expand kernel flushes them once at its end) instead of one global atomic per action and warp.
-template <bool CTA_ACTIONS = false>
-__device__ __forceinline__ void insert_row(const Params& p, const State& s, uint64_t meta, bool valid, const Prefetched& f,
+template <bool CTA_ACTIONS = false, bool XS = false>
+__device__ __forceinline__ void insert_row(const Params& p, const State& s, uint64_t meta, bool valid, const Prefetched<XS>& f,
                                             unsigned& probes, unsigned& oom, int& failed, uint32_t act_smem = 0) {
   bool is_new = false;
   if (valid) {
     if (f.inmodel) {
-      int r = set_insert_pre(p.table, p.bucket_mask, f.id, f.bk, probes);
-      if (r < 0) failed = KMC_FAIL_TABLE_FULL;
+      int r;
+      if constexpr (XS) {
+        r = xset_insert(p.table, p.bucket_mask, f.id.fp, f.key, f.bk, probes);
+        if (r < 0) failed = r == -1 ? KMC_FAIL_TABLE_FULL : KMC_FAIL_SET_TIMEOUT;
+      } else {
+        r = set_insert_pre(p.table, p.bucket_mask, f.id, f.bk, probes);
+        if (r < 0) failed = KMC_FAIL_TABLE_FULL;
+      }
       is_new = r > 0;
     } else {
       ++oom;
@@ -568,6 +723,7 @@ static constexpr int CTA_CTR_BYTES = (CTA_ACTION + M::NUM_ACTIONS) * 8;
 // its registers are not live across the bodies.  Called by all 32 lanes of a warp (n is warp-uniform).
 // It gets the kernel parameters it reads by value, in registers: with a `const Params&` argument the caller kept a copy
 // of Params in local memory and the insert reached every pointer through a generic load ahead of its first probe.
+template <bool XS = false>
 __device__ __noinline__ int insert_stage(void* table, uint64_t bucket_mask, uint64_t* store, uint64_t* parent,
                                          uint64_t max_states, uint64_t store_mask, uint64_t store_base, DevCounters* ctr,
                                          uint64_t* viol_ring, uint32_t wbuf, unsigned n, uint32_t cta) {
@@ -592,8 +748,8 @@ __device__ __noinline__ int insert_stage(void* table, uint64_t bucket_mask, uint
 #pragma unroll
     for (int k = 0; k < W; ++k) s.w[k] = lds64(row + k * 8);
     const uint64_t meta = lds64(row + W * 8);
-    const Prefetched f = prefetch_row(p, s, valid);
-    insert_row<true>(p, s, meta, valid, f, probes, oom, failed, cta + CTA_ACTION * 8);
+    const Prefetched<XS> f = prefetch_row<XS>(p, s, valid);
+    insert_row<true, XS>(p, s, meta, valid, f, probes, oom, failed, cta + CTA_ACTION * 8);
   }
   probes = __reduce_add_sync(0xffffffffu, probes);
   oom = __reduce_add_sync(0xffffffffu, oom);
@@ -602,6 +758,17 @@ __device__ __noinline__ int insert_stage(void* table, uint64_t bucket_mask, uint
     if (oom) reds_add64(cta + CTA_OOM * 8, oom);
   }
   return failed;
+}
+
+// insert_stage of a warp's n staged rows at `wbuf`, into the set form the context uses
+__device__ __forceinline__ int insert_stage_of(const Params& p, uint32_t wbuf, unsigned n, uint32_t cta) {
+  if constexpr (XS_ON) {
+    if (p.exact)
+      return insert_stage<XS_ON>(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
+                                 p.viol_ring, wbuf, n, cta);
+  }
+  return insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
+                      p.viol_ring, wbuf, n, cta);
 }
 
 // called by all 32 lanes of a warp at a converged point
@@ -613,8 +780,7 @@ __device__ __forceinline__ void flush_stage(const Params& p, uint32_t wbuf, uint
   if (n == 0 || (!force && n < (unsigned)STAGE_FLUSH)) return;
   unsigned lane = lane_id();
   if (p.fused) {
-    const int f = insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
-                               p.viol_ring, wbuf, n, cta);
+    const int f = insert_stage_of(p, wbuf, n, cta);
     if (f) failed = f;
   } else if (p.world == 1) {
     unsigned long long base = 0;
@@ -1009,6 +1175,21 @@ __device__ __forceinline__ void load_row(State& s, uint64_t& meta, const uint64_
   }
 }
 
+template <bool XS = false>
+__device__ __forceinline__ void insert_rows(const Params& p, const uint64_t* rows, uint64_t n, unsigned& probes, unsigned& oom,
+                                            int& failed) {
+  const uint64_t n_round = (n + 31) & ~31ull;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+    const bool v0 = i < n;
+    State s0;
+    uint64_t m0;
+    load_row(s0, m0, rows, i, v0);
+    const Prefetched<XS> f0 = prefetch_row<XS>(p, s0, v0);
+    insert_row<false, XS>(p, s0, m0, v0, f0, probes, oom, failed);
+  }
+}
+
 // One candidate row per thread per iteration.  (Two rows per thread -- two sectors in flight per
 // lane -- was measured slower: 72 vs 63 ms on the 340 M-state model; the extra registers cost more
 // occupancy than the added memory-level parallelism gains.)
@@ -1023,15 +1204,11 @@ __global__ void __launch_bounds__(256) k_insert(Params p, const uint64_t* rows, 
     n = p.region_rows;
     failed = KMC_FAIL_CAND_FULL;
   }
-  const uint64_t n_round = (n + 31) & ~31ull;
-  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
-    const bool v0 = i < n;
-    State s0;
-    uint64_t m0;
-    load_row(s0, m0, rows, i, v0);
-    Prefetched f0 = prefetch_row(p, s0, v0);
-    insert_row(p, s0, m0, v0, f0, probes, oom, failed);
+  if constexpr (XS_ON) {
+    if (p.exact) insert_rows<XS_ON>(p, rows, n, probes, oom, failed);
+    else insert_rows(p, rows, n, probes, oom, failed);
+  } else {
+    insert_rows(p, rows, n, probes, oom, failed);
   }
   for (int o = 16; o > 0; o >>= 1) {
     probes += __shfl_xor_sync(0xffffffffu, probes, o);
@@ -1129,8 +1306,7 @@ __global__ void __launch_bounds__(INIT_BLOCK) k_init(Params p, int branch, uint6
     cands += count - base < 32 ? count - base : 32;
     if (staged >= (unsigned)STAGE_FLUSH) {
       __syncwarp();
-      const int f = insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
-                                 p.viol_ring, wbuf, staged, cta);
+      const int f = insert_stage_of(p, wbuf, staged, cta);
       if (f) failed = f;
       staged = 0;
       __syncwarp();
@@ -1138,8 +1314,7 @@ __global__ void __launch_bounds__(INIT_BLOCK) k_init(Params p, int branch, uint6
   }
   if (staged) {
     __syncwarp();
-    const int f = insert_stage(p.table, p.bucket_mask, p.store, p.parent, p.max_states, p.store_mask, p.store_base, p.ctr,
-                               p.viol_ring, wbuf, staged, cta);
+    const int f = insert_stage_of(p, wbuf, staged, cta);
     if (f) failed = f;
   }
   layout = __reduce_or_sync(0xffffffffu, layout);
@@ -1294,7 +1469,7 @@ __global__ void __launch_bounds__(256) k_insert_inbox(Params p) {
       for (int k = 0; k < W; ++k) s0.w[k] = __ldcs(row + k);
       m0 = __ldcs(row + W);
     }
-    Prefetched f0 = prefetch_row(p, s0, v0);
+    const Prefetched<> f0 = prefetch_row(p, s0, v0);
     insert_row(p, s0, m0, v0, f0, probes, oom, failed);
   }
   for (int o = 16; o > 0; o >>= 1) {
@@ -1371,6 +1546,16 @@ __global__ void __launch_bounds__(256) k_rebuild(Params p, const uint64_t* state
 #pragma unroll
     for (int k = 0; k < W; ++k) s.w[k] = states[i * W + k];
     unsigned probes = 0;
+    if constexpr (XS_ON) {
+      if (p.exact) {
+        State key;
+        uint64_t fp;
+        state_xident(s, key, fp);
+        const int r = xset_insert(p.table, p.bucket_mask, fp, key, ld_xbucket(p.table, bucket_of(fp, p.bucket_mask)), probes);
+        if (r < 0) failed = r == -1 ? KMC_FAIL_TABLE_FULL : KMC_FAIL_SET_TIMEOUT;
+        continue;
+      }
+    }
     if (set_insert(p.table, p.bucket_mask, state_ident(s), probes) < 0) failed = KMC_FAIL_TABLE_FULL;
   }
   if (failed) atomicCAS(&p.ctr->fail, 0ull, (unsigned long long)failed);
@@ -1404,6 +1589,7 @@ __global__ void k_fpset_put(void* table, uint64_t bucket_mask, const uint64_t* f
 // found in host memory already) and the host empties the table.  The filter (k_set_mark, then k_set_compact) removes
 // from the states appended since the last filter those whose key is in host memory: they were found in an earlier epoch.
 static constexpr int KEY_WORDS = SLOT_BYTES / 8;
+static constexpr int XKEY_WORDS = W;          // exact_set: a key in host memory is the (canonical) packed state
 static constexpr int SET_TILE = 256;          // states per tile of the filter's compaction
 
 // The identity a stored key stands for: the key alone gives the fingerprint that picks its bucket.
@@ -1430,21 +1616,31 @@ __device__ __forceinline__ bool marked(const unsigned* marks, long long slot) {
 }
 
 // Slots [first, first + n) of the table: every key that is not marked goes to `out`, compacted with ballot/popc (the
-// order does not matter), counted in ctr->set_count.
+// order does not matter), counted in ctr->set_count.  XS (exact_set): a key is the W state words behind a slot's
+// header (XKEY_WORDS), and a slot is full when its header is not XEMPTY.
+template <bool XS = false>
 __global__ void __launch_bounds__(256) k_set_flush(const void* table, uint64_t first, uint64_t n, const unsigned* marks,
                                                     uint64_t* out, DevCounters* ctr) {
+  constexpr int KW = XS ? XKEY_WORDS : KEY_WORDS;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const unsigned lane = lane_id();
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ((n + 31) & ~31ull); i += stride) {
     const uint64_t slot = first + i;
-    uint64_t k[KEY_WORDS];
+    uint64_t k[KW];
     bool take = false;
     if (i < n) {
-      const uint64_t* src = static_cast<const uint64_t*>(table) + slot * KEY_WORDS;
+      if constexpr (XS) {
+        const uint64_t* src = static_cast<const uint64_t*>(table) + slot * XSLOT_WORDS;
 #pragma unroll
-      for (int w = 0; w < KEY_WORDS; ++w) k[w] = src[w];
-      const bool full = KEY128 ? (k[0] & k[KEY_WORDS - 1]) != ~0ull : k[0] != 0;
-      take = full && !marked(marks, (long long)slot);
+        for (int w = 0; w < KW; ++w) k[w] = src[1 + w];
+        take = src[0] != XEMPTY && !marked(marks, (long long)slot);
+      } else {
+        const uint64_t* src = static_cast<const uint64_t*>(table) + slot * KEY_WORDS;
+#pragma unroll
+        for (int w = 0; w < KEY_WORDS; ++w) k[w] = src[w];
+        const bool full = KEY128 ? (k[0] & k[KEY_WORDS - 1]) != ~0ull : k[0] != 0;
+        take = full && !marked(marks, (long long)slot);
+      }
     }
     const unsigned who = __ballot_sync(0xffffffffu, take);
     if (!who) continue;
@@ -1452,19 +1648,28 @@ __global__ void __launch_bounds__(256) k_set_flush(const void* table, uint64_t f
     if ((int)lane == __ffs(who) - 1) base = atomicAdd(&ctr->set_count, (unsigned long long)__popc(who));
     base = __shfl_sync(0xffffffffu, base, __ffs(who) - 1);
     if (take) {
-      uint64_t* dst = out + (base + __popc(who & ((1u << lane) - 1))) * KEY_WORDS;
+      uint64_t* dst = out + (base + __popc(who & ((1u << lane) - 1))) * KW;
 #pragma unroll
-      for (int w = 0; w < KEY_WORDS; ++w) dst[w] = k[w];
+      for (int w = 0; w < KW; ++w) dst[w] = k[w];
     }
   }
 }
 
 // n host keys (one chunk of the stream through HBM): each one found in the table marks its slot.
+template <bool XS = false>
 __global__ void __launch_bounds__(256) k_set_mark(const void* table, uint64_t bucket_mask, const uint64_t* keys, uint64_t n,
                                                    unsigned* marks) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long slot = set_contains(table, bucket_mask, key_ident(keys + i * KEY_WORDS));
+    long long slot;
+    if constexpr (XS) {
+      State key;
+#pragma unroll
+      for (int w = 0; w < W; ++w) key.w[w] = keys[i * XKEY_WORDS + w];
+      slot = xset_contains(table, bucket_mask, fingerprint(key), key);
+    } else {
+      slot = set_contains(table, bucket_mask, key_ident(keys + i * KEY_WORDS));
+    }
     if (slot >= 0) atomicOr(marks + (slot >> 5), 1u << (slot & 31));
   }
 }
@@ -1485,7 +1690,20 @@ __global__ void __launch_bounds__(SET_TILE) k_set_compact(Params p, uint64_t fir
       State s;
 #pragma unroll
       for (int k = 0; k < W; ++k) s.w[k] = p.store[g * W + k];
-      kept = !marked(marks, set_contains(p.table, p.bucket_mask, state_ident(s)));
+      long long slot = -1;
+      if constexpr (XS_ON) {
+        if (p.exact) {
+          State key;
+          uint64_t fp;
+          state_xident(s, key, fp);
+          slot = xset_contains(p.table, p.bucket_mask, fp, key);
+        } else {
+          slot = set_contains(p.table, p.bucket_mask, state_ident(s));
+        }
+      } else {
+        slot = set_contains(p.table, p.bucket_mask, state_ident(s));
+      }
+      kept = !marked(marks, slot);
       keep[j] = kept ? 1 : 0;
       if (!kept) {
         const uint64_t meta = p.parent[g];
@@ -1604,7 +1822,9 @@ struct Engine {
   // set_spill (single rank): the keys of the set move to host memory whenever the table would pass set_limit(); the
   // filter's marks (a bit per table slot) and its staging and compaction space live at the end and the start of `cand`
   bool set_spill = false;
-  // the keys in host memory, KEY_WORDS words each as the table stores them: one block of exactly its size per flushed
+  // exact_set (single rank) on a model whose key is hashed: the set's key is the packed state (XSLOT_WORDS slots)
+  bool exact = false;
+  // the keys in host memory, key_words() words each as the table stores them: one block of exactly its size per flushed
   // slot range, so that the array grows without the copies (and the transient double size) of a growing vector
   std::vector<std::vector<uint64_t>> host_keys;
   uint64_t set_host_keys = 0;           // keys in host_keys
@@ -1618,7 +1838,7 @@ struct Engine {
   cudaEvent_t set_copied[2] = {}, set_probed[2] = {};
 
   void* table = nullptr;
-  uint64_t table_slots = 0;             // slots of SLOT_BYTES each
+  uint64_t table_slots = 0;             // slots of slot_bytes() each
   uint64_t* store = nullptr;
   uint64_t* parent = nullptr;
   uint64_t* cand = nullptr;
@@ -1669,10 +1889,16 @@ struct Engine {
   uint64_t level_first = 0, level_count = 0, level = 0;
   std::string last_error;
 
+  uint64_t slot_bytes() const { return exact ? XSLOT_BYTES : SLOT_BYTES; }
+  uint64_t bucket_mask() const { return table_slots / (exact ? XBUCKET_SLOTS : BUCKET_SLOTS) - 1; }
+  uint64_t key_words() const { return exact ? XKEY_WORDS : KEY_WORDS; }      // a key in host memory (set_spill)
+  // the table's empty fill: all-ones 16-byte keys and exact_set headers, zero 8-byte fingerprints
+  int empty_byte() const { return KEY128 || exact ? 0xFF : 0; }
+
   Params params() const {
     Params p;
     p.table = table;
-    p.bucket_mask = table_slots / BUCKET_SLOTS - 1;
+    p.bucket_mask = bucket_mask();
     p.store = store;
     p.parent = parent;
     p.max_states = max_states;
@@ -1690,6 +1916,7 @@ struct Engine {
     p.p2p = 0;
     p.inbox_buf = inbox_buf;
     p.fused = 0;
+    p.exact = exact ? 1 : 0;
     return p;
   }
 };
@@ -1811,7 +2038,7 @@ static int engine_alloc(Engine& E) {
   const uint64_t per_state = (uint64_t)W * 8 + 8;
   if (E.table_log2 == 0 && E.max_states == 0) {
     int lg = 34;
-    while (lg > 16 && ((uint64_t)SLOT_BYTES << lg) + (uint64_t)((1ull << lg) / 2.5) * per_state > budget) --lg;
+    while (lg > 16 && (E.slot_bytes() << lg) + (uint64_t)((1ull << lg) / 2.5) * per_state > budget) --lg;
     E.table_log2 = lg;
     E.max_states = (uint64_t)((1ull << lg) / 2.5);
   } else if (E.table_log2 == 0) {
@@ -1826,7 +2053,7 @@ static int engine_alloc(Engine& E) {
   }
   E.table_slots = 1ull << E.table_log2;
   if (E.max_states == 0) {
-    const uint64_t table_bytes = E.table_slots * SLOT_BYTES;
+    const uint64_t table_bytes = E.table_slots * E.slot_bytes();
     const uint64_t room = budget > table_bytes ? (budget - table_bytes) / per_state : 0;
     E.max_states = std::max<uint64_t>(1024, std::min<uint64_t>(E.table_slots / 2, room));
     if (E.spill) {
@@ -1844,7 +2071,7 @@ static int engine_alloc(Engine& E) {
   if (E.fanout_bound == 0) E.fanout_bound = std::min<uint32_t>((uint32_t)M::MAX_FANOUT, 32u);
   E.chunk_states = std::max<uint64_t>(1, E.region_rows / E.fanout_bound);
   if (E.own_stream) CK(cudaStreamCreateWithFlags(&E.stream, cudaStreamNonBlocking));
-  CK(cudaMalloc(&E.table, E.table_slots * SLOT_BYTES));
+  CK(cudaMalloc(&E.table, E.table_slots * E.slot_bytes()));
   CK(cudaMalloc(&E.store, E.max_states * W * 8));
   CK(cudaMalloc(&E.parent, E.max_states * 8));
   CK(cudaMalloc(&E.cand, E.region_rows * E.world * ROW * 8));
@@ -1888,9 +2115,9 @@ static int set_alloc(Engine& E) {
     E.last_error = "set_spill: the candidate buffer cannot hold the filter's marks and working space (raise cand_bytes)";
     return KMC_E_BADARG;
   }
-  E.set_stage_keys = std::min<uint64_t>(1 << 20, set_scratch_words(E) / (2 * KEY_WORDS));
+  E.set_stage_keys = std::min<uint64_t>(1 << 20, set_scratch_words(E) / (2 * E.key_words()));
   for (int b = 0; b < 2; ++b) {
-    CK(cudaHostAlloc(&E.set_pinned[b], E.set_stage_keys * SLOT_BYTES, cudaHostAllocDefault));
+    CK(cudaHostAlloc(&E.set_pinned[b], E.set_stage_keys * E.key_words() * 8, cudaHostAllocDefault));
     CK(cudaEventCreateWithFlags(&E.set_copied[b], cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&E.set_probed[b], cudaEventDisableTiming));
   }
@@ -1916,27 +2143,29 @@ static int read_tail(Engine& E, uint64_t* tail, uint64_t* fail) {
 // KMC_E_OOM.
 static int set_flush(Engine& E) {
   TimedLaunch t(E, 3);
-  const uint64_t range = set_scratch_words(E) / KEY_WORDS;
+  const uint64_t KW = E.key_words();
+  const uint64_t range = set_scratch_words(E) / KW;
   for (uint64_t s0 = 0; s0 < E.table_slots; s0 += range) {
     const uint64_t n = std::min(range, E.table_slots - s0);
     CK(cudaMemsetAsync(&E.ctr->set_count, 0, sizeof(unsigned long long), E.stream));
-    k_set_flush<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, s0, n, set_marks(E), E.cand, E.ctr);
+    if (E.exact) k_set_flush<XS_ON><<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, s0, n, set_marks(E), E.cand, E.ctr);
+    else k_set_flush<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, s0, n, set_marks(E), E.cand, E.ctr);
     CK(cudaGetLastError());
     unsigned long long k = 0;
     CK(cudaMemcpyAsync(&k, &E.ctr->set_count, sizeof(k), cudaMemcpyDeviceToHost, E.stream));
     CK(cudaStreamSynchronize(E.stream));
     if (k == 0) continue;
     try {
-      E.host_keys.emplace_back(k * KEY_WORDS);
+      E.host_keys.emplace_back(k * KW);
     } catch (const std::bad_alloc&) {
       E.last_error = "set_spill: host memory for the fingerprint set's keys is exhausted";
       return KMC_E_OOM;
     }
-    CK(cudaMemcpy(E.host_keys.back().data(), E.cand, k * SLOT_BYTES, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(E.host_keys.back().data(), E.cand, k * KW * 8, cudaMemcpyDeviceToHost));
     E.set_host_keys += k;
-    E.set_link_bytes += k * SLOT_BYTES;
+    E.set_link_bytes += k * KW * 8;
   }
-  CK(cudaMemsetAsync(E.table, KEY128 ? 0xFF : 0, E.table_slots * SLOT_BYTES, E.stream));
+  CK(cudaMemsetAsync(E.table, E.empty_byte(), E.table_slots * E.slot_bytes(), E.stream));
   CK(cudaMemsetAsync(set_marks(E), 0, set_mark_words(E) * 8, E.stream));
   E.set_keys = 0;
   E.set_from = E.set_tail;
@@ -1947,29 +2176,30 @@ static int set_flush(Engine& E) {
 // Marks the slot of every table key that is in host memory: the host keys stream through two pinned buffers into two
 // staging areas of the scratch space, the copy of one chunk (on its own stream) overlapping the probes of the previous.
 static int set_mark(Engine& E) {
-  const uint64_t S = E.set_stage_keys;
-  uint64_t* stage[2] = {E.cand, E.cand + S * KEY_WORDS};
-  const uint64_t bucket_mask = E.table_slots / BUCKET_SLOTS - 1;
+  const uint64_t S = E.set_stage_keys, KW = E.key_words();
+  uint64_t* stage[2] = {E.cand, E.cand + S * KW};
+  const uint64_t bucket_mask = E.bucket_mask();
   // the staging areas are free once the work already on the engine stream (which may use the scratch space) is done
   for (int b = 0; b < 2; ++b) CK(cudaEventRecord(E.set_probed[b], E.stream));
   uint64_t k = 0;
   for (const std::vector<uint64_t>& block : E.host_keys) {
-    const uint64_t nkeys = block.size() / KEY_WORDS;
+    const uint64_t nkeys = block.size() / KW;
     for (uint64_t i = 0; i < nkeys; i += S, ++k) {
       const int b = (int)(k & 1);
       const uint64_t n = std::min(S, nkeys - i);
       CK(cudaEventSynchronize(E.set_probed[b]));          // the probes of chunk k - 2 are done with buffer b
-      memcpy(E.set_pinned[b], block.data() + i * KEY_WORDS, n * SLOT_BYTES);
+      memcpy(E.set_pinned[b], block.data() + i * KW, n * KW * 8);
       CK(cudaStreamWaitEvent(E.set_copy_stream, E.set_probed[b], 0));
-      CK(cudaMemcpyAsync(stage[b], E.set_pinned[b], n * SLOT_BYTES, cudaMemcpyHostToDevice, E.set_copy_stream));
+      CK(cudaMemcpyAsync(stage[b], E.set_pinned[b], n * KW * 8, cudaMemcpyHostToDevice, E.set_copy_stream));
       CK(cudaEventRecord(E.set_copied[b], E.set_copy_stream));
       CK(cudaStreamWaitEvent(E.stream, E.set_copied[b], 0));
-      k_set_mark<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, bucket_mask, stage[b], n, set_marks(E));
+      if (E.exact) k_set_mark<XS_ON><<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, bucket_mask, stage[b], n, set_marks(E));
+      else k_set_mark<<<grid_for(E, n, 256, 8), 256, 0, E.stream>>>(E.table, bucket_mask, stage[b], n, set_marks(E));
       CK(cudaGetLastError());
       CK(cudaEventRecord(E.set_probed[b], E.stream));
     }
   }
-  E.set_link_bytes += E.set_host_keys * SLOT_BYTES;
+  E.set_link_bytes += E.set_host_keys * KW * 8;
   return KMC_OK;
 }
 
@@ -2060,7 +2290,7 @@ static int inv_begin(Engine& E, bool complete) {
 
 static int engine_reset(Engine& E) {
   CK(cudaSetDevice(E.device));
-  CK(cudaMemsetAsync(E.table, KEY128 ? 0xFF : 0, E.table_slots * SLOT_BYTES, E.stream));      // empty marker: all-ones keys / zero fingerprints
+  CK(cudaMemsetAsync(E.table, E.empty_byte(), E.table_slots * E.slot_bytes(), E.stream));
   DevCounters h;
   memset(&h, 0, sizeof(h));
   CK(cudaMemcpyAsync(E.ctr, &h, sizeof(h), cudaMemcpyHostToDevice, E.stream));
@@ -2097,7 +2327,7 @@ static void publish(Engine& E, const DevCounters& h, bool clamp) {
   st.out_of_model = h.out_of_model;
   st.probes = h.probes;
   st.table_slots = E.table_slots;
-  st.slot_bytes = SLOT_BYTES;
+  st.slot_bytes = E.slot_bytes();
   st.max_states = E.max_states;
   st.set_flushes = E.set_flushes;
   st.set_host_keys = E.set_host_keys;
@@ -2128,6 +2358,7 @@ static int fail_to_error(unsigned long long f) {
     case KMC_FAIL_STORE_FULL: return KMC_E_STORE_FULL;
     case KMC_FAIL_CAND_FULL: return KMC_E_CAND_FULL;
     case KMC_FAIL_PEER_TIMEOUT: return KMC_E_PEER_TIMEOUT;
+    case KMC_FAIL_SET_TIMEOUT: return KMC_E_SET_TIMEOUT;
     default: return KMC_E_CUDA;
   }
 }
@@ -2756,7 +2987,17 @@ static int multi_run(kmcm_ctx* c);
 static constexpr const char* DEVICE_INIT_ONE_GPU =
     "this model's Init is enumerated on the GPU (device Init), which runs on one GPU: no \"gpus\" > 1, no world > 1, "
     "no kmc_shard_* calls";
+// An exact_set context keys its set by the packed state, which the exchange of fingerprint-sharded rows and the
+// fingerprint-only kmc_fpset_* calls do not carry.
+static constexpr const char* EXACT_SET_ONE_GPU =
+    "exact_set runs on one GPU: no \"gpus\" > 1, no world > 1, no kmc_shard_* calls";
+static constexpr const char* EXACT_SET_NO_FPSET =
+    "exact_set keys the set by the packed state: a 64-bit fingerprint is not a key of it (no kmc_fpset_* calls)";
 static bool shard_refused(Engine& e) {
+  if (e.exact) {
+    e.last_error = EXACT_SET_ONE_GPU;
+    return true;
+  }
 #ifdef KMC_HAS_DEVICE_INIT
   e.last_error = DEVICE_INIT_ONE_GPU;
   return true;
@@ -2786,6 +3027,7 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
   if (json_num(options_json, "stop_after_states", &d)) E.stop_after_states = (uint64_t)d;
   if (json_bool(options_json, "spill", &b)) E.spill = b;
   if (json_bool(options_json, "set_spill", &b)) E.set_spill = b;
+  if (json_bool(options_json, "exact_set", &b)) E.exact = b && !EXACT_SET;      // (an exact key already: nothing to do)
   json_str(options_json, "checkpoint_dir", &E.checkpoint_dir);
   json_str(options_json, "recover", &E.recover_dir);
   if (json_num(options_json, "checkpoint_minutes", &d)) E.checkpoint_minutes = d;
@@ -2808,6 +3050,11 @@ int kmcm_create(const char* options_json, kmcm_ctx** out) {
     return KMC_E_BADARG;
   }
 #endif
+  if (E.exact && (gpus || E.world > 1)) {
+    E.last_error = EXACT_SET_ONE_GPU;
+    *out = c;
+    return KMC_E_BADARG;
+  }
   if (E.set_spill && (gpus || E.world > 1)) {
     // each rank's set would need the keys of the others' host memory too
     E.last_error = "set_spill runs on one GPU (no \"gpus\" > 1, no world > 1)";
@@ -2858,7 +3105,7 @@ void kmcm_destroy(kmcm_ctx* c) {
   delete c;
 }
 
-int kmcm_model_info(const kmcm_ctx*, kmc_model_info_t* out) {
+int kmcm_model_info(const kmcm_ctx* c, kmc_model_info_t* out) {
   if (!out) return KMC_E_BADARG;
   memset(out, 0, sizeof(*out));
   out->words = W;
@@ -2871,7 +3118,7 @@ int kmcm_model_info(const kmcm_ctx*, kmc_model_info_t* out) {
 #endif
   out->max_fanout = M::MAX_FANOUT;
   out->check_deadlock = M::CHECK_DEADLOCK;
-  out->exact = EXACT_SET ? 1 : 0;
+  out->exact = (EXACT_SET || (c && E.exact)) ? 1 : 0;
   strncpy(out->name, KMC_MODEL_NAME, sizeof(out->name) - 1);
   strncpy(out->digest, KMC_MODEL_DIGEST, sizeof(out->digest) - 1);
   return KMC_OK;
@@ -3082,6 +3329,7 @@ const char* kmcm_strerror(const kmcm_ctx* c, int code) {
     case KMC_E_NO_GPU: return "no CUDA device visible; this library has no CPU fallback";
     case KMC_E_CAND_FULL: return "candidate buffer overflow (raise cand_bytes or fanout_bound)";
     case KMC_E_PEER_TIMEOUT: return "a peer rank did not arrive at a device-side synchronisation point within 30 s";
+    case KMC_E_SET_TIMEOUT: return "exact_set: a claimed slot of the set was not published in time";
     default: return "unknown error";
   }
 }
@@ -3089,7 +3337,8 @@ const char* kmcm_strerror(const kmcm_ctx* c, int code) {
 // ---- fingerprint set alone ---------------------------------------------------------------
 // (not with set_spill: the keys in host memory are not consulted, so put() could call a known fingerprint new)
 static int fpset_call(kmcm_ctx* c, const uint64_t* fps, size_t n, uint8_t* out, int insert) {
-  if (!c || E.set_spill || (!fps && n) || (!out && n)) return KMC_E_BADARG;
+  if (c && E.exact) E.last_error = EXACT_SET_NO_FPSET;
+  if (!c || E.set_spill || E.exact || (!fps && n) || (!out && n)) return KMC_E_BADARG;
   if (n == 0) return KMC_OK;
   CK(cudaSetDevice(E.device));
   uint64_t* d_fps = nullptr;
@@ -3110,7 +3359,8 @@ int kmcm_fpset_put(kmcm_ctx* c, const uint64_t* fps, size_t n, uint8_t* out_seen
 int kmcm_fpset_contains(kmcm_ctx* c, const uint64_t* fps, size_t n, uint8_t* out) { return fpset_call(c, fps, n, out, 0); }
 int kmcm_fpset_size(const kmcm_ctx* c_, uint64_t* out) {
   kmcm_ctx* c = const_cast<kmcm_ctx*>(c_);
-  if (!c || E.set_spill || !out) return KMC_E_BADARG;
+  if (c && E.exact) E.last_error = EXACT_SET_NO_FPSET;
+  if (!c || E.set_spill || E.exact || !out) return KMC_E_BADARG;
   unsigned long long t = 0;
   CK(cudaSetDevice(E.device));
   CK(cudaMemcpy(&t, &E.ctr->store_tail, 8, cudaMemcpyDeviceToHost));
@@ -3367,7 +3617,7 @@ int kmcm_shard_level_sync(kmcm_ctx* c, uint64_t* board_out) {
     E.stats.generated = mine[4];
     E.stats.deadlocks = mine[6];
     E.stats.table_slots = E.table_slots;
-    E.stats.slot_bytes = SLOT_BYTES;
+    E.stats.slot_bytes = E.slot_bytes();
     E.stats.max_states = E.max_states;
     if (E.level_count) E.widths.push_back(E.level_count);
     E.stats.levels = E.stats.depth = E.widths.size();

@@ -23,7 +23,7 @@ BUILD = os.path.join(ROOT, "build")
 KMC_ERRORS = {
     0: "KMC_OK", -1: "KMC_E_BADARG", -2: "KMC_E_CUDA", -3: "KMC_E_OOM", -4: "KMC_E_TABLE_FULL",
     -5: "KMC_E_STORE_FULL", -6: "KMC_E_LAYOUT_OVERFLOW", -7: "KMC_E_MODEL", -8: "KMC_E_STATE", -9: "KMC_E_NO_GPU",
-    -10: "KMC_E_CAND_FULL", -11: "KMC_E_PEER_TIMEOUT",
+    -10: "KMC_E_CAND_FULL", -11: "KMC_E_PEER_TIMEOUT", -12: "KMC_E_SET_TIMEOUT",
 }
 
 
@@ -211,8 +211,8 @@ class RunResult:
 
 class Checker:
     """One GPU-resident model checker instance (one ``kmc_ctx``).  ``options`` are kmc_create's JSON options
-    (include/kspecmc.h), e.g. ``table_log2=27, max_states=N, spill=True, set_spill=True``; ``cont`` stands for
-    ``continue``."""
+    (include/kspecmc.h), e.g. ``table_log2=27, max_states=N, spill=True, set_spill=True, exact_set=True``; ``cont``
+    stands for ``continue``."""
 
     def __init__(self, model: str, model_lib: str | None = None, model_json: str | None = None, **options):
         self.lib = load_library()

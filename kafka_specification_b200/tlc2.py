@@ -2,7 +2,7 @@
 
     python -m kafka_specification_b200.tlc2 [-config F.cfg] [-workers N|auto] [-deadlock] [-continue]
                                              [-fpbits N] [-maxstates N] [-I dir] [-metadir d] [-checkpoint MIN]
-                                             [-recover DIR] [-spill] [-setspill] [-coverage N] [-tool]
+                                             [-recover DIR] [-spill] [-setspill] [-exactset] [-coverage N] [-tool]
                                              [-dump FILE | -dump dot[,actionlabels][,colorize][,snapshot] FILE] SPEC
 
 ``SPEC`` is a module name or a path to ``SPEC.tla``; modules it EXTENDS / INSTANCEs are resolved
@@ -16,6 +16,9 @@ messages in TLC's tool-mode markers (``@!@!@STARTMSG code:class @!@!@`` ... ``@!
 run (also after a violation): TLC repeats it every N minutes, but a search here takes seconds.
 ``-setspill`` (an extension, like ``-spill``) moves the fingerprint set's keys to host memory whenever its table fills,
 so that a state space larger than the table still finishes (one GPU; see ``set_spill`` in include/kspecmc.h).
+``-exactset`` (an extension as well) keys the fingerprint set by the packed state itself instead of a hashed
+fingerprint, so that "No error has been found" is exact on every model (one GPU; see ``exact_set`` in
+include/kspecmc.h); the collision estimate is then 0.  Models whose key is exact already are unchanged by it.
 ``-continue`` searches past violations and prints one error block per violated invariant, ordered by (first violating
 level, cfg index), each with the counterexample that ends in the smallest-fingerprint violator of that level; the first
 block is the one a run without ``-continue`` prints.  TLC under ``-continue`` prints a trace for every violating state
@@ -65,6 +68,8 @@ def parse_args(argv):
                     help="extension: keep only the live BFS window in HBM and move older levels to host memory")
     ap.add_argument("-setspill", action="store_true",
                     help="extension: move the fingerprint set's keys to host memory whenever its HBM table fills")
+    ap.add_argument("-exactset", action="store_true",
+                    help="extension: key the fingerprint set by the packed state itself (no fingerprint collisions)")
     ap.add_argument("-tool", action="store_true")
     ap.add_argument("-device", type=int, default=0)
     ap.add_argument("-cleanup", action="store_true")
@@ -241,6 +246,8 @@ def main(argv=None) -> int:
         opts["spill"] = True
     if a.setspill:
         opts["set_spill"] = True
+    if a.exactset:
+        opts["exact_set"] = True
     try:
         ck = Checker(name, **opts)
     except KmcError as e:
@@ -275,7 +282,9 @@ def main(argv=None) -> int:
         msg("success", "Model checking completed. No error has been found.\n"
                        "  Estimates of the probability that TLC did not check all reachable states\n"
                        "  because two distinct states had the same fingerprint:")
-        if ck.info.exact:
+        if a.exactset and ck.info.exact:
+            msg("collision", "  calculated (optimistic):  val = 0 (exact: the set key is the packed state)")
+        elif ck.info.exact:
             msg("collision", "  calculated (optimistic):  val = 0 (the set key is a bijection of the packed state: exact)")
         else:
             p128 = collision_probability(r.distinct, r.generated) / 2.0 ** 65
