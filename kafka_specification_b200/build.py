@@ -199,12 +199,28 @@ def device_init_registry() -> dict:
     return models
 
 
+ARITH_REGISTRY = os.path.join(TEST_SPECS_DIR, "MODELS_arith.json")
+
+
+def arith_registry() -> dict:
+    """The models that test lowered integer arithmetic past 32 bits (tests/specs/MODELS_arith.json): build_all()
+    compiles them too.  Like device_init_registry(), they are kept out of registry() and its pinned headers."""
+    if not os.path.exists(ARITH_REGISTRY):
+        return {}
+    with open(ARITH_REGISTRY) as f:
+        models = json.load(f)
+    clash = (set(registry()) | set(device_init_registry())) & set(models)
+    if clash:
+        raise RuntimeError(f"models registered twice: {sorted(clash)}")
+    return models
+
+
 def build_all(force: bool = False, only: list[str] | None = None, verbose: bool = True, jobs: int = 0) -> dict[str, str]:
     """Lower (sequentially, it is fast) and compile (in parallel: nvcc dominates) every registered model."""
     from concurrent.futures import ThreadPoolExecutor
     build_dispatcher(force)
     todo = []
-    for name, spec in {**registry(), **device_init_registry()}.items():
+    for name, spec in {**registry(), **device_init_registry(), **arith_registry()}.items():
         if only and name not in only:
             continue
         module, cfg_path = spec["module"], os.path.join(ROOT, spec["cfg"])

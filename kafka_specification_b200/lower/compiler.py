@@ -26,8 +26,38 @@ from ..frontend.modules import ModuleContext
 from ..frontend.tla_parser import Def
 from ..frontend.values import FnVal, fmt, sort_key
 from . import layout as L
-from .svals import (SYMBOLIC, LowerError, SAtom, SBool, SFn, SInt, SLazy, SRec, SSeq, SSet, SUnion,
-                    is_atom_const, is_const, is_int_const, is_static, kind_sig)
+from .svals import (INT32_MAX, INT64_MAX, INT64_MIN, SYMBOLIC, LowerError, SAtom, SBool, SFn, SInt, SLazy, SRec, SSeq,
+                    SSet, SUnion, c_int, fits_int, is_atom_const, is_const, is_int_const, is_static, kind_sig)
+
+RANGE_ENUM_MAX = 1 << 16       # members of an `a .. b` that the lowering enumerates; a wider one stays a pair of bounds
+
+
+def expr_text(e, depth: int = 0) -> str:
+    """A short rendering of an expression for error messages."""
+    if depth > 3:
+        return "..."
+    k = e[0]
+    if k in ("num", "bool"):
+        return str(e[1]).upper() if k == "bool" else str(e[1])
+    if k == "str":
+        return f'"{e[1]}"'
+    if k == "id":
+        return e[1]
+    if k == "app":
+        return f"{e[1]}(" + ", ".join(expr_text(x, depth + 1) for x in e[2]) + ")"
+    if k == "binop":
+        return f"{expr_text(e[2], depth + 1)} {e[1]} {expr_text(e[3], depth + 1)}"
+    if k == "neg":
+        return f"-{expr_text(e[1], depth + 1)}"
+    if k == "prime":
+        return f"{expr_text(e[1], depth + 1)}'"
+    if k == "if":
+        return f"IF {expr_text(e[1], depth + 1)} THEN {expr_text(e[2], depth + 1)} ELSE {expr_text(e[3], depth + 1)}"
+    if k == "quant":
+        return f"\\{e[1]} ... : {expr_text(e[3], depth + 1)}"
+    if k == "subset":
+        return f"SUBSET {expr_text(e[1], depth + 1)}"
+    return f"<{k} expression>"
 
 
 class UnpinnedRef(Exception):
@@ -192,8 +222,32 @@ class Lowerer:
         return self.gids[a]
 
     # ------------------------------------------------------------- C helpers
-    def tmp_int(self, e: str) -> str:
-        return self.cg.tmp("int", e) if len(e) > self.TMP_THRESHOLD else e
+    def tmp_int(self, e: str, lo: int = 0, hi: int = 0) -> str:
+        """``e`` (in a temporary when it is long) as a C integer that holds every value of [lo, hi]: an ``int`` where
+        they fit one, else an ``int64_t``."""
+        if len(e) <= self.TMP_THRESHOLD:
+            return e
+        return self.cg.tmp("int" if fits_int(lo, hi) else "int64_t", e)
+
+    @staticmethod
+    def int_ctype(lo: int, hi: int, what) -> str:
+        """The C type of an integer expression with values in [lo, hi]; LowerError beyond 64-bit integers."""
+        if lo < INT64_MIN or hi > INT64_MAX:
+            raise LowerError(f"the integer expression {what() if callable(what) else what} takes values in {lo} .. {hi}, "
+                             f"beyond 64-bit integers")
+        return "int" if fits_int(lo, hi) else "int64_t"
+
+    @staticmethod
+    def wide(A) -> str:
+        """The C text of the SInt A as a 64-bit operand, which makes a binary operation on it 64-bit (an SInt outside
+        the range of ``int`` is 64-bit already)."""
+        return f"(int64_t){A.s}" if fits_int(A.lo, A.hi) else A.s
+
+    def tmp_code(self, ty, e: str) -> str:
+        """A layout code of type ``ty``: an ``int``, or a ``uint64_t`` for a type with more codes than an ``int`` holds."""
+        if ty.card - 1 <= INT32_MAX:
+            return self.tmp_int(e)
+        return self.cg.tmp("uint64_t", e) if len(e) > self.TMP_THRESHOLD else e
 
     def tmp_uint(self, e: str) -> str:
         return self.cg.tmp("unsigned", e) if len(e) > self.TMP_THRESHOLD else e
@@ -305,7 +359,7 @@ class Lowerer:
             ea = self.encode(ty, a)
             eb = self.encode(ty, b)
             if len(self.traps) == marks:          # no range traps were needed for either branch
-                code = self.tmp_int(f"({c.s} ? {ea} : {eb})")
+                code = self.tmp_code(ty, f"({c.s} ? {ea} : {eb})")
                 self.remember_code(ty, v, code)
                 return code
             del self.traps[marks:]
@@ -316,13 +370,29 @@ class Lowerer:
         if isinstance(v, SInt):
             return v
         if is_int_const(v):
-            return SInt(str(v), v, v)
+            return SInt(c_int(v), v, v)
         raise LowerError(f"expected an integer, got {v!r}")
 
-    def mk_int(self, s: str, lo: int, hi: int):
+    def mk_int(self, s: str, lo: int, hi: int, what="an integer expression"):
+        self.int_ctype(lo, hi, what)
         if lo == hi:
             return lo
-        return SInt(self.tmp_int(s), lo, hi)
+        return SInt(self.tmp_int(s, lo, hi), lo, hi)
+
+    def arith(self, op: str, A: SInt, B: SInt, what="an integer expression"):
+        """A op B (op one of + - *) in the C type its operands and its result need: in ``int`` when all three fit one,
+        else in ``int64_t``, so that no intermediate value wraps."""
+        if op == "+":
+            lo, hi = A.lo + B.lo, A.hi + B.hi
+        elif op == "-":
+            lo, hi = A.lo - B.hi, A.hi - B.lo
+        else:
+            c = [A.lo * B.lo, A.lo * B.hi, A.hi * B.lo, A.hi * B.hi]
+            lo, hi = min(c), max(c)
+        self.int_ctype(lo, hi, what)
+        if fits_int(lo, hi) and fits_int(A.lo, A.hi) and fits_int(B.lo, B.hi):
+            return self.mk_int(f"({A.s} {op} {B.s})", lo, hi, what)
+        return self.mk_int(f"({self.wide(A)} {op} {B.s})", lo, hi, what)
 
     def atom_expr(self, v) -> str:
         if isinstance(v, SAtom):
@@ -490,7 +560,8 @@ class Lowerer:
             A, B = self.as_sint(a), self.as_sint(b)
             if A.s == B.s:
                 return a
-            return SInt(self.tmp_int(f"({c.s} ? {A.s} : {B.s})"), min(A.lo, B.lo), max(A.hi, B.hi))
+            lo, hi = min(A.lo, B.lo), max(A.hi, B.hi)
+            return SInt(self.tmp_int(f"({c.s} ? {A.s} : {B.s})", lo, hi), lo, hi)
         if ka == "bool":
             return self.b_ite(c, a, b)
         if ka == "atom":
@@ -551,6 +622,10 @@ class Lowerer:
         raise LowerError(f"not a set: {s!r}")
 
     def enumerate_lazy(self, s: SLazy) -> list:
+        if s.kind == "range":
+            what = f"{s.a} .. {s.b}" if is_const(s.a) and is_const(s.b) else "a run-time range"
+            raise LowerError(f"{what} may hold more than {RANGE_ENUM_MAX} integers: too many to enumerate "
+                             f"(it can only be tested for membership)")
         if s.kind == "recset":
             names = list(s.a)
             cols = []
@@ -617,7 +692,7 @@ class Lowerer:
             return self.b_or([self.b_and([g, self.member(v, s)]) for g, v in x.alts])
         if isinstance(s, frozenset) and isinstance(x, SInt):
             ints = sorted(v for v in s if is_int_const(v))
-            if ints and ints == list(range(ints[0], ints[-1] + 1)):
+            if ints and ints[-1] - ints[0] + 1 == len(ints):          # contiguous (the members are distinct)
                 return self.b_and([self.cmp(">=", x, ints[0]), self.cmp("<=", x, ints[-1])])
             return self.b_or([self.cmp("==", x, v) for v in ints])
         return self.b_or([self.b_and([g, self.eq(x, e)]) for g, e in self.set_items(s)])
@@ -628,6 +703,8 @@ class Lowerer:
         k = kind_sig(x)
         if s.kind == "nat":
             return self.cmp(">=", x, 0) if k == "int" else False
+        if s.kind == "range":
+            return self.b_and([self.cmp(">=", x, s.a), self.cmp("<=", x, s.b)]) if k == "int" else False
         if s.kind == "int":
             return k == "int"
         if s.kind == "recset":
@@ -674,9 +751,15 @@ class Lowerer:
         return self.b_and([self.b_or([self.b_not(g), self.member(e, b)]) for g, e in self.set_items(a)])
 
     def interval(self, a, b):
+        """a .. b: the set itself while it has at most RANGE_ENUM_MAX members, else its bounds (an SLazy "range"), which
+        membership and layout types use as they are and which is refused where it would have to be enumerated."""
         if is_int_const(a) and is_int_const(b):
+            if b - a + 1 > RANGE_ENUM_MAX:
+                return SLazy("range", a, b)
             return frozenset(range(a, b + 1))
         A, B = self.as_sint(a), self.as_sint(b)
+        if B.hi - A.lo + 1 > RANGE_ENUM_MAX:
+            return SLazy("range", a, b)
         return SSet([(self.b_and([self.cmp("<=", a, k), self.cmp("<=", k, b)]), k) for k in range(A.lo, B.hi + 1)])
 
     # ------------------------------------------------------------ sequences / tuples (module Sequences)
@@ -970,6 +1053,8 @@ class Lowerer:
                     sv = self.ev(e[2][0], ctx, fm, env, S)
                     if isinstance(sv, frozenset):
                         return len(sv)
+                    if isinstance(sv, SLazy) and sv.kind == "range" and is_const(sv.a) and is_const(sv.b):
+                        return max(0, sv.b - sv.a + 1)
                     items = self.distinct_items(sv)
                     fixed = sum(1 for g, _ in items if g is True)
                     dyn = [g for g, _ in items if g is not True]
@@ -1003,7 +1088,10 @@ class Lowerer:
             if is_int_const(v):
                 return -v
             A = self.as_sint(v)
-            return self.mk_int(f"(-{A.s})", -A.hi, -A.lo)
+            what = lambda: expr_text(e)
+            self.int_ctype(-A.hi, -A.lo, what)
+            return self.mk_int(f"(-{A.s})" if fits_int(A.lo, A.hi) and fits_int(-A.hi, -A.lo) else f"(-{self.wide(A)})",
+                               -A.hi, -A.lo, what)
         if k == "binop":
             return self.ev_binop(e, ctx, fm, env, S)
         if k == "if":
@@ -1162,13 +1250,7 @@ class Lowerer:
                 a = self.narrow_union(a, "int")
             if isinstance(b, SUnion):
                 b = self.narrow_union(b, "int")
-            A, B = self.as_sint(a), self.as_sint(b)
-            if op == "+":
-                return self.mk_int(f"({A.s} + {B.s})", A.lo + B.lo, A.hi + B.hi)
-            if op == "-":
-                return self.mk_int(f"({A.s} - {B.s})", A.lo - B.hi, A.hi - B.lo)
-            c = [A.lo * B.lo, A.lo * B.hi, A.hi * B.lo, A.hi * B.hi]
-            return self.mk_int(f"({A.s} * {B.s})", min(c), max(c))
+            return self.arith(op, self.as_sint(a), self.as_sint(b), lambda: expr_text(e))
         if op in ("\\div", "%"):
             # Integers: floor division and the modulus with a positive divisor (TLA+ defines a % b only for b > 0)
             if isinstance(a, SUnion):
@@ -1182,12 +1264,24 @@ class Lowerer:
             A, B = self.as_sint(a), self.as_sint(b)
             if B.lo <= 0:
                 raise LowerError(f"{op}: the divisor may be non-positive ({B.lo}..{B.hi})")
+            what = lambda: expr_text(e)
+            # with a negative dividend, C's truncating / and % are corrected through -a + b - 1 (\div) or (a % b) + b (%):
+            # the C type is chosen from the operands, those intermediate values and the result
             if op == "\\div":
                 c = [A.lo // B.lo, A.lo // B.hi, A.hi // B.lo, A.hi // B.hi]
-                e = f"({A.s} / {B.s})" if A.lo >= 0 else f"(({A.s}) >= 0 ? ({A.s}) / ({B.s}) : -((-({A.s}) + ({B.s}) - 1) / ({B.s})))"
-                return self.mk_int(e, min(c), max(c))
-            e = f"({A.s} % {B.s})" if A.lo >= 0 else f"(((({A.s}) % ({B.s})) + ({B.s})) % ({B.s}))"
-            return self.mk_int(e, 0, min(B.hi - 1, A.hi) if A.lo >= 0 else B.hi - 1)
+                lo, hi = min(c), max(c)
+                mid = (0, 0) if A.lo >= 0 else (max(1, -A.hi) + B.lo - 1, -A.lo + B.hi - 1)
+            else:
+                lo, hi = 0, min(B.hi - 1, A.hi) if A.lo >= 0 else B.hi - 1
+                mid = (0, 0) if A.lo >= 0 else (B.lo - B.hi + 1, 2 * B.hi - 1)
+            self.int_ctype(*mid, what)
+            narrow = all(fits_int(*r) for r in ((A.lo, A.hi), (B.lo, B.hi), mid, (lo, hi)))
+            sa, sb = (A.s, B.s) if narrow else (self.wide(A), B.s)
+            if op == "\\div":
+                code = f"({sa} / {sb})" if A.lo >= 0 else f"(({sa}) >= 0 ? ({sa}) / ({sb}) : -((-({sa}) + ({sb}) - 1) / ({sb})))"
+            else:
+                code = f"({sa} % {sb})" if A.lo >= 0 else f"(((({sa}) % ({sb})) + ({sb})) % ({sb}))"
+            return self.mk_int(code, lo, hi, what)
         if op == "..":
             return self.interval(a, b)
         if op == "\\o":
@@ -1733,6 +1827,9 @@ class Lowerer:
         out = []
         for a in self.layout.atoms:
             sh = f" >> {a.shift}" if a.shift else ""
+            if a.bits > 32:
+                out.append(f"  [[maybe_unused]] const uint64_t a{a.index} = (s.w[{a.word}]{sh}) & 0x{a.mask:x}ull;  // {a.path}")
+                continue
             out.append(f"  [[maybe_unused]] const unsigned a{a.index} = (unsigned)((s.w[{a.word}]{sh}) & 0x{a.mask:x}ull);"
                        f"  // {a.path}")
         return out

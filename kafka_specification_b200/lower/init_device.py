@@ -22,32 +22,11 @@ from __future__ import annotations
 
 from ..frontend.values import sort_key
 from .compiler import CG, Closure, Marker, UnpinnedRef, render
-from .svals import LowerError, SBool, SFn, SInt, SLazy, SRec, SSet, is_const, is_int_const, kind_sig
+from .compiler import expr_text as _text
+from .svals import LowerError, SBool, SFn, SInt, SLazy, SRec, SSet, c_int, fits_int, is_const, is_int_const, kind_sig
 
 INIT_DEVICE_THRESHOLD = 65536          # Init candidates above which Init is enumerated on the GPU without the cfg hint
 MAX_BRANCH_CANDIDATES = 1 << 40        # candidate space of one branch (~10^12): beyond it the device form is refused
-
-
-def _text(e, depth: int = 0) -> str:
-    """A short rendering of an expression for error messages."""
-    if depth > 3:
-        return "..."
-    k = e[0]
-    if k in ("num", "bool"):
-        return str(e[1]).upper() if k == "bool" else str(e[1])
-    if k == "str":
-        return f'"{e[1]}"'
-    if k == "id":
-        return e[1]
-    if k == "app":
-        return f"{e[1]}(" + ", ".join(_text(x, depth + 1) for x in e[2]) + ")"
-    if k == "binop":
-        return f"{_text(e[2], depth + 1)} {e[1]} {_text(e[3], depth + 1)}"
-    if k == "quant":
-        return f"\\{e[1]} ... : {_text(e[3], depth + 1)}"
-    if k == "subset":
-        return f"SUBSET {_text(e[1], depth + 1)}"
-    return f"<{k} expression>"
 
 
 class DeviceInit:
@@ -151,6 +130,8 @@ class DeviceInit:
             return {"set"}
         if s.kind == "cross":
             return {"tuple"}
+        if s.kind == "range":
+            return {"int"}
         raise LowerError(f"Init conjunct '{_text(conj)}': cannot decode a generator over {s.kind}")
 
     def card(self, s, conj) -> int:
@@ -159,6 +140,8 @@ class DeviceInit:
             return len(s)
         if not isinstance(s, SLazy):
             raise LowerError(f"Init conjunct '{_text(conj)}': the generator set is not a constant set")
+        if s.kind == "range" and is_int_const(s.a) and is_int_const(s.b):
+            return max(0, s.b - s.a + 1)
         if s.kind in ("nat", "int", "seq"):
             name = {"nat": "Nat", "int": "Int", "seq": "Seq(S)"}[s.kind]
             raise LowerError(f"Init conjunct '{_text(conj)}': a generator over {name} is unbounded")
@@ -213,6 +196,14 @@ class DeviceInit:
         ctype = "unsigned" if radix <= (1 << 32) else "uint64_t"
         return self.lw.cg.tmp(ctype, f"({ctype})({e})")
 
+    def _int_range(self, x: str, lo: int, hi: int) -> SInt:
+        """Member number x of lo .. hi: in `int` arithmetic where the members and x fit one, else in `int64_t`."""
+        if fits_int(lo, hi) and hi - lo <= (1 << 31) - 1:
+            e = f"((int){x} + {lo})" if lo else f"(int){x}"
+        else:
+            e = f"((int64_t){x} + {c_int(lo)})" if lo else f"(int64_t){x}"
+        return SInt(self.lw.tmp_int(e, lo, hi), lo, hi)
+
     def decode(self, s, x: str, conj):
         """The symbolic member number x (a C expression in [0, card(s))) of the constant set s."""
         lw = self.lw
@@ -221,13 +212,14 @@ class DeviceInit:
             items = sorted(s, key=sort_key)
             if len(items) == 1:
                 return items[0]
-            if all(is_int_const(v) for v in items) and items == list(range(items[0], items[-1] + 1)):
-                lo = items[0]
-                return SInt(lw.tmp_int(f"((int){x} + {lo})" if lo else f"(int){x}"), lo, items[-1])
+            if all(is_int_const(v) for v in items) and items[-1] - items[0] + 1 == len(items):
+                return self._int_range(x, items[0], items[-1])
             res = items[-1]
             for i in range(len(items) - 2, -1, -1):
                 res = lw.mux(SBool(lw.tmp_bool(f"({x} == {i}u)")), items[i], res)
             return res
+        if s.kind == "range":
+            return self._int_range(x, s.a, s.b)
         if s.kind in ("recset", "cross"):
             parts = list(s.a.values()) if s.kind == "recset" else list(s.a)
             vals, stride = [], 1

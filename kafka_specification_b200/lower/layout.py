@@ -6,7 +6,7 @@ of the type tree are *atoms*: unsigned bit-fields that never straddle a word.
 
 Type            encoding
 --------------  -----------------------------------------------------------------------------
-TInt(lo, hi)    code = value - lo
+TInt(lo, hi)    code = value - lo; the one type whose atom may be wider than 32 bits (up to 63: read as int64_t)
 TEnum(atoms)    code = index of the model value / string in the (gid-sorted) universe
 TUnion(alts)    code = offset(alt) + alt code          (records[o] is a record or Nil, FiniteReplicatedLog.tla:41-44)
 TRec / TFn      product of the members: separate atoms at top level, mixed radix when nested in a set/union
@@ -31,8 +31,8 @@ from __future__ import annotations
 
 from ..frontend.cfg import ModelValue
 from ..frontend.values import FnVal, fmt, sort_key
-from .svals import (LowerError, SAtom, SBool, SFn, SInt, SRec, SSeq, SSet, SUnion, is_atom_const,
-                    is_const, is_int_const, kind_sig)
+from .svals import (INT32_MAX, INT64_MAX, INT64_MIN, LowerError, SAtom, SBool, SFn, SInt, SRec, SSeq, SSet, SUnion,
+                    c_int, fits_int, is_atom_const, is_const, is_int_const, kind_sig)
 
 
 def bits_for(card: int) -> int:
@@ -99,9 +99,10 @@ class Layout:
         lay.words, lay.bits = desc["words"], desc["bits"]
         return lay
 
-    def new_atom(self, path: str, bits: int, card: int | None = None) -> Atom:
-        if bits > 32:
-            raise LowerError(f"atom {path} needs {bits} bits (> 32)")
+    def new_atom(self, path: str, bits: int, card: int | None = None, max_bits: int = 32) -> Atom:
+        """A new atom; only an integer field may be wider than 32 bits (its code is computed in 64-bit arithmetic)."""
+        if bits > max_bits:
+            raise LowerError(f"atom {path} needs {bits} bits (> {max_bits})")
         a = Atom(len(self.atoms), path, bits, card)
         self.atoms.append(a)
         return a
@@ -216,9 +217,9 @@ class Ty:
             return
         out[self.atom.index] = lw.encode(self, v)
 
-    def _alloc_scalar(self, lay: Layout, path: str):
+    def _alloc_scalar(self, lay: Layout, path: str, max_bits: int = 32):
         b = bits_for(self.card)
-        self.atom = lay.new_atom(path, b, self.card) if b > 0 else None
+        self.atom = lay.new_atom(path, b, self.card, max_bits) if b > 0 else None
 
 
 class TInt(Ty):
@@ -234,7 +235,13 @@ class TInt(Ty):
         return {"t": "int", "lo": self.lo, "hi": self.hi}
 
     def alloc(self, lay, path):
-        self._alloc_scalar(lay, path)
+        if not INT64_MIN < self.lo <= self.hi <= INT64_MAX:
+            raise LowerError(f"integer field {path} ranges over {self.lo} .. {self.hi}, beyond 64-bit integers")
+        self._alloc_scalar(lay, path, max_bits=63)
+
+    def narrow(self) -> bool:
+        """Do the values and the codes of this field fit a C `int`?  (Else they are read as `int64_t`.)"""
+        return fits_int(self.lo, self.hi) and self.card - 1 <= INT32_MAX
 
     def py_enc(self, v):
         if not is_int_const(v) or not (self.lo <= v <= self.hi):
@@ -253,11 +260,18 @@ class TInt(Ty):
             raise LowerError(f"cannot store {v!r} in an integer field")
         if v.lo < self.lo or v.hi > self.hi:
             lw.trap_unless(lw.b_and([lw.cmp(">=", v, self.lo), lw.cmp("<=", v, self.hi)]))
-        return lw.tmp_int(f"({v.s} - {self.lo})" if self.lo else v.s)
+        if fits_int(v.lo, v.hi) and fits_int(v.lo - self.lo, v.hi - self.lo):
+            return lw.tmp_int(f"({v.s} - {self.lo})" if self.lo else v.s)
+        if not self.lo:
+            return lw.tmp_int(v.s, v.lo, v.hi)
+        # in 64-bit unsigned arithmetic, where the code of a value that traps (and is never stored) cannot overflow
+        return lw.tmp_code(self, f"((uint64_t){v.s} - 0x{self.lo & ((1 << 64) - 1):x}ull)")
 
     def dec(self, lw, code):
         if self.card == 1:
             return self.lo
+        if not self.narrow():
+            return SInt(f"((int64_t){code} + {c_int(self.lo)})" if self.lo else f"(int64_t){code}", self.lo, self.hi)
         return SInt(f"((int){code} + {self.lo})" if self.lo else f"(int){code}", self.lo, self.hi)
 
 

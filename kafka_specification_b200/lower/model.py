@@ -80,6 +80,8 @@ class TypeInference:
     def type_from_setval(self, v) -> L.Ty:
         lw = self.lw
         if isinstance(v, SLazy):
+            if v.kind == "range" and is_int_const(v.a) and is_int_const(v.b):
+                return L.TInt(v.a, v.b)
             if v.kind == "recset":
                 return L.TRec({f: self.type_from_setval(s) for f, s in v.a.items()})
             if v.kind == "fnset":

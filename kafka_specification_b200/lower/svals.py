@@ -11,7 +11,7 @@ are C expression strings over the unpacked state atoms.
   SRec   record with symbolic fields          SFn   function over a constant finite domain
   SSet   guarded element list [(guard, elem)] -- the set of elems whose guard holds
   SUnion value of one of several kinds [(guard, value)], guards mutually exclusive
-  SLazy  non-enumerated constant set descriptor (record sets, function sets, SUBSET, Nat, Seq(S), S \\X T)
+  SLazy  non-enumerated set descriptor (record sets, function sets, SUBSET, Nat, Seq(S), S \\X T, a wide a .. b)
   SSeq   sequence / tuple: a length (int or SInt) and ``cap`` item values; item i (0-based) is meaningful
          iff i < length.  A fully constant sequence is a Python tuple.
 """
@@ -23,6 +23,22 @@ from ..frontend.values import FnVal
 
 class LowerError(Exception):
     pass
+
+
+INT32_MIN, INT32_MAX = -(1 << 31), (1 << 31) - 1
+INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
+
+
+def fits_int(lo: int, hi: int) -> bool:
+    """Does every value of [lo, hi] fit a C `int`?"""
+    return INT32_MIN <= lo and hi <= INT32_MAX
+
+
+def c_int(v: int) -> str:
+    """The C literal of an integer constant (the most negative int64_t has none: -2^63 + 1 would be its negation)."""
+    if not INT64_MIN <= v <= INT64_MAX:
+        raise LowerError(f"the integer {v} is beyond 64-bit integers")
+    return "(-9223372036854775807ll - 1)" if v == INT64_MIN else str(v)
 
 
 class SInt:
@@ -115,7 +131,7 @@ class SLazy:
     __slots__ = ("kind", "a", "b")
 
     def __init__(self, kind: str, a=None, b=None):
-        self.kind, self.a, self.b = kind, a, b   # 'nat' | 'int' | 'recset'(a=dict) | 'fnset'(a=dom,b=rng) | 'powerset'(a=base) | 'union'(a,b) | 'seq'(a=elem set) | 'cross'(a=[sets])
+        self.kind, self.a, self.b = kind, a, b   # 'nat' | 'int' | 'recset'(a=dict) | 'fnset'(a=dom,b=rng) | 'powerset'(a=base) | 'union'(a,b) | 'seq'(a=elem set) | 'cross'(a=[sets]) | 'range'(a=lo, b=hi: int or SInt)
 
     def __repr__(self):
         return f"SLazy({self.kind}, {self.a}, {self.b})"

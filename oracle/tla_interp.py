@@ -591,6 +591,12 @@ class Interp:
         op = e[1]
         if op == "=>":
             return (not self.ev_bool(e[2], ctx, fm, env, st, st1)) or self.ev_bool(e[3], ctx, fm, env, st, st1)
+        if op in ("\\in", "\\notin") and e[3][0] == "binop" and e[3][1] == "..":
+            # x \in lo .. hi by its bounds: the same truth value without building a set of up to 2^40 integers
+            x = self.ev(e[2], ctx, fm, env, st, st1)
+            lo, hi = self.ev_int(e[3][2], ctx, fm, env, st, st1), self.ev_int(e[3][3], ctx, fm, env, st, st1)
+            inside = not isinstance(x, bool) and isinstance(x, int) and lo <= x <= hi
+            return inside if op == "\\in" else not inside
         a = self.ev(e[2], ctx, fm, env, st, st1)
         b = self.ev(e[3], ctx, fm, env, st, st1)
         if op == "=":

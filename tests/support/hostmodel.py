@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
-from kafka_specification_b200.build import device_init_registry, registry, tla_search_dirs  # noqa: E402
+from kafka_specification_b200.build import arith_registry, device_init_registry, registry, tla_search_dirs  # noqa: E402
 from kafka_specification_b200.lower.model import LoweredModel, lower_model  # noqa: E402,F401
 
 BUILD = os.path.join(ROOT, "build", "hosttest")
@@ -87,9 +87,9 @@ def _library_path(header_text: str, invariants_text: str) -> str:
 
 @functools.lru_cache(maxsize=None)
 def lower_registered(name: str) -> LoweredModel:
-    """The registered model `name` (build.registry() or build.device_init_registry()) lowered from its module and cfg
-    as build() lowers it, once per process; `lower_registered.__wrapped__(name)` lowers it afresh."""
-    spec = {**registry(), **device_init_registry()}[name]
+    """The registered model `name` (build.registry(), build.device_init_registry() or build.arith_registry()) lowered from
+    its module and cfg as build() lowers it, once per process; `lower_registered.__wrapped__(name)` lowers it afresh."""
+    spec = {**registry(), **device_init_registry(), **arith_registry()}[name]
     with open(os.path.join(ROOT, spec["cfg"])) as f:
         return lower_model(spec["module"], tla_search_dirs(), f.read(), name=name)
 
